@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — denoised frames/s of the ray-trace + SVGF hot path on N B200s (one process per GPU).
+"""bench.py — denoised frames/s of the ray-trace + SVGF hot path on N H100s (one process per GPU).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {1,2,3,4,5}] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {1,2,3,4,5}] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one frame of the configuration's passes.  --config picks one of BASELINE.json's five configurations as
 SURVEY.md §8d makes them concrete; the default is the largest single-GPU one, config 3:
@@ -18,7 +18,7 @@ steps between barrier + synchronize, max over ranks):
   value     frames/s with the G-buffer resident in HBM (static camera, steady state: history saturated; the blue-noise sample
             index advances every frame so the traced rays change every frame).  N > 1: the frame is split into row bands and the
             final output is all-gathered to every rank INSIDE the timed region (value_distributed = without the gather)
-  pan       the same passes over a 40-frame lateral camera pan (0.05 units / frame): the G-buffer is produced on the device
+  pan       the same passes over a K-frame lateral camera pan (0.05 units / frame): the G-buffer is produced on the device
             every frame by hr_gbuffer_render (its time is reported separately), reprojection follows real motion vectors
   e2e       frames/s from HOST inputs to HOST outputs, every step: the host builds the 496-byte hr_frame (camera, light,
             matrices) -> hr_gbuffer_render on the device (SURVEY.md §8 f1: the G-buffer is produced where the reference
@@ -33,14 +33,19 @@ steps between barrier + synchronize, max over ranks):
   post_passes   (N = 1, informational, own process) deferred combine -> TAA -> tone map and the ground-truth path tracer at the bench
             resolution: ms per launch, roofline fractions on their algorithmic bytes (36 / 12 B/px), Mrays/s of the path tracer
   cpu_baseline / --impl reference   the CPU oracle (a port: the reference has no CPU path and cannot be built here),
-            OpenMP over all host threads (set explicitly), best of 5 frames on a 1/16-area render of the same workload
-            (same scene and passes), stated as frames/s of that SAMPLE and extrapolated x16 in `value`
+            OpenMP over all host threads (set explicitly), best of 5 frames (--impl reference: of K frames) on a 1/4-area render
+            (1/16 at 8K) of the same workload (same scene and passes), stated as frames/s of that SAMPLE and extrapolated in `value`
 
-Inputs (G-buffer 199 MB + history / intermediates > 300 MB per 4K frame) exceed the 126 MB L2: "inputs_larger_than_l2".
+Inputs (G-buffer 199 MB + history / intermediates > 300 MB per 4K frame) exceed the 50 MB L2: "inputs_larger_than_l2".
+
+--dump-outputs DIR (GPU arm, rank 0): after the timed steps of `value`, the final output of every pass as the last timed step left it,
+as DIR/<pass>.npy in its stored layout: half-float images as float32 (H x W x channels); integer images as float64, which holds every
+uint32 exactly — at 1 spp without denoising the final output is the packed R32_UINT visibility mask, one word per 8x4 pixel block
+(ceil(H/4) x ceil(W/8), bit (y & 3) * 8 + (x & 7)).  An image larger than its share of 60 MB is reduced to a fixed sample of its
+elements (seed 0, sorted flat indices, elements x channels), so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
-import glob
 import json
 import os
 import sys
@@ -78,20 +83,7 @@ def read_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def read_traffic(kernel_key):
-    """DRAM bytes per launch of the roofline kernel from the newest committed ncu summary (profiles/*_traffic.json)."""
-    best = None
-    for p in sorted(glob.glob(os.path.join(ROOT, "profiles", "*_traffic.json"))):
-        try:
-            d = json.load(open(p))
-        except Exception:
-            continue
-        if kernel_key in d:
-            best = (d[kernel_key], os.path.relpath(p, ROOT), d.get("_source"))
-    return best
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -144,7 +136,7 @@ def cpu_model():
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU arm
-def oracle_fps(cfg, scale_div=None, frames=5):
+def oracle_fps(cfg, scale_div=None, frames=5, time_limit=120.0):
     """The CPU oracle on a 1/scale_div^2-area render of the configuration (same scene, passes, parameters): best of `frames`
     individually timed steady-state frames with every host thread.  Returns a dict for `cpu_baseline`."""
     import oracle as O
@@ -209,13 +201,13 @@ def oracle_fps(cfg, scale_div=None, frames=5):
         t0 = time.perf_counter()
         one(f)
         times.append(time.perf_counter() - t0)
-        if time.perf_counter() - t_all > 120.0:
+        if time_limit is not None and time.perf_counter() - t_all > time_limit:
             break
     best = min(times)
     return {"value": 1.0 / (best * extrap), "unit": "frames/s", "cores": int(O.lib().orc_num_threads()), "kind": "port", "cpu_model": cpu_model(),
             "sample": f"{sw}x{shh} render ({'1/%d' % int(round(extrap)) if extrap > 1 else 'full'} area) of the same scene and passes, best of {len(times)} frames "
                       f"(each {', '.join('%.2f' % t for t in times)} s), sample rate {1.0 / best:.3f} frames/s" + (f", extrapolated x{extrap:.0f}" if extrap > 1 else ""),
-            "sample_frames_per_s": 1.0 / best, "extrapolation": extrap}
+            "sample_frames_per_s": 1.0 / best, "extrapolation": extrap, "frames": len(times)}
 
 
 def refl_params(cfg):
@@ -296,6 +288,20 @@ class Rig:
 
 def texel_bytes(img):
     return {1: 4, 2: 2, 3: 4, 4: 8, 5: 1}[img.format]
+
+
+def dump_outputs(out_dir, rig, stream, budget=60_000_000):
+    """--dump-outputs: the final output of every pass as <pass>.npy; see the module docstring."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = budget // len(rig.passes)
+    for name, p in rig.passes.items():
+        a = p.download(100, stream)
+        a = a.astype(np.float64 if a.dtype.kind in "ui" else np.float32)
+        if a.nbytes > share:
+            flat = a.reshape(a.shape[0] * a.shape[1], -1)
+            idx = np.sort(np.random.default_rng(0).choice(flat.shape[0], share // (a.itemsize * flat.shape[1]), replace=False))
+            a = flat[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------------------------- post-pass leg
@@ -425,7 +431,10 @@ def main():
     ap.add_argument("--config", type=int, default=3, choices=sorted(CONFIGS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the pan / dense-K5 / host-G-buffer legs (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the final outputs of the last timed step as DIR/<pass>.npy (GPU arm)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU arm (--impl ours)")
     cfg = CONFIGS[args.config]
     W, H = cfg["W"], cfg["H"]
     rank = int(os.environ.get("RANK", "0"))
@@ -440,8 +449,8 @@ def main():
         # this arm times the CPU oracle, a port, with every host thread on a bounded sample of the same workload.
         if rank != 0:
             return
-        cb = oracle_fps(cfg, frames=max(1, min(args.steps, 5)))
-        line = {"metric": metric, "value": cb["value"], "unit": "frames/s", "n_gpus": args.gpus, "steps": max(1, min(args.steps, 5)), "warmup": 1,
+        cb = oracle_fps(cfg, frames=max(1, args.steps), time_limit=None)
+        line = {"metric": metric, "value": cb["value"], "unit": "frames/s", "n_gpus": args.gpus, "steps": cb["frames"], "warmup": 1,
                 "ms_per_step": 1000.0 / cb["value"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32 (fp16 storage)", "data": "synthetic",
                 "config": config, "impl": "reference", "cpu_baseline": cb,
                 "note": "cpu oracle (port), measured on a reduced-area sample and extrapolated; NOT the upstream implementation (it has no CPU path)",
@@ -553,6 +562,8 @@ def main():
     rig.stats(stream)  # reset the ray counters
     r_val = timed(step_resident, args.steps, profile=True, sample=True)
     st_val = rig.stats(stream)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, rig, stream)
     r_dist = None
     if world > 1:
         gather(False)
@@ -640,7 +651,7 @@ def main():
         for _ in range(8):
             step_pan()
         ge0, ge1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        r_pan = timed(step_pan, 40, profile=True)
+        r_pan = timed(step_pan, args.steps, profile=True)
         # the G-buffer producer alone
         barrier()
         ge0.record()
@@ -651,7 +662,7 @@ def main():
                 ctx.gbuffer_render(state["f"].ping_pong, state["f"], 0, 0, stream)
         ge1.record()
         torch.cuda.synchronize()
-        extras["pan"] = {"frames": 40, "step_world_units": PAN_STEP, "ms": r_pan["ms"], "gbuffer_ms_per_frame": ge0.elapsed_time(ge1) / 10.0, "stages": r_pan["stages"]}
+        extras["pan"] = {"frames": args.steps, "step_world_units": PAN_STEP, "ms": r_pan["ms"], "gbuffer_ms_per_frame": ge0.elapsed_time(ge1) / 10.0, "stages": r_pan["stages"]}
         # ---- host G-buffer mode of the e2e leg (upload GB2 + GB3 + depth every frame; GB1 is not read by these passes) -----------------
         if world == 1:
             gh = pyhr.GBufferHost(W, H, pinned=True)
@@ -669,8 +680,8 @@ def main():
             ctx.check(ctx.lib.hr_gbuffer_stage_upload(ctx.h, C.byref(gh_desc)), "hr_gbuffer_stage_upload")
             for _ in range(3):
                 step_e2e_host()
-            r_host = timed(step_e2e_host, min(args.steps, 20), finish=lambda: cur.wait_event(ev_copied))
-            extras["e2e_host_gbuffer"] = {"value": min(args.steps, 20) / (r_host["ms"] / 1e3), "h2d_bytes_per_step": W * H * 20}
+            r_host = timed(step_e2e_host, args.steps, finish=lambda: cur.wait_event(ev_copied))
+            extras["e2e_host_gbuffer"] = {"value": args.steps / (r_host["ms"] / 1e3), "h2d_bytes_per_step": W * H * 20}
             ctx.check(ctx.lib.hr_gbuffer_commit_staged(ctx.h, state["f"].ping_pong, C.c_void_p(stream)), "hr_gbuffer_commit_staged")
             torch.cuda.synchronize()
 
@@ -732,7 +743,7 @@ def main():
         torch.cuda.synchronize()
         ctx.set_profiling(True)
         shp.stage_times()
-        for i in range(20):
+        for i in range(args.steps):
             fd = pyhr.make_frame(DENSE_CAM[0], DENSE_CAM[1], W, H, prev=fd, num_frames=42 + i, light=light)
             shp.render(fd, stream)
         torch.cuda.synchronize()
@@ -779,12 +790,10 @@ def main():
             on, tot = s.tiles_denoise, max(1, s.tiles_total)
             proc = 64.0 * (on * b_on + (tot - on) * b_off)
             contract = b_on * s.pixels_total
-            tr = read_traffic(key)
             roof = {"kernel": kname, "bound": "hbm", "achieved": proc / 1e9 / (at_ms / 1e3), "peak": peak, "unit": "GB/s", "frac": proc / 1e9 / (at_ms / 1e3) / peak,
                     "frac_contract": contract / 1e9 / (at_ms / 1e3) / peak, "avg_launch_ms": at_ms, "per_iteration_ms": at,
                     "algorithmic_bytes_per_launch": proc, "contract_bytes_per_launch": contract, "bytes_per_px": {"denoise_tile": b_on, "other_tile": b_off},
-                    "tiles_total": int(tot), "tiles_on_denoise_list": int(on), "peak_source": peak_src,
-                    "traffic": tr[0] if (tr and world == 1) else None, "traffic_source": (f"{tr[1]} ({tr[2]})" if tr else None)}
+                    "tiles_total": int(tot), "tiles_on_denoise_list": int(on), "peak_source": peak_src}
         rays = {k: {"primary_per_frame": s.rays_primary / max(1, s.renders), "secondary_per_frame": s.rays_secondary / max(1, s.renders),
                     "trace_kernel_ms": r_val["stages"].get(k, {}).get("Ray Trace"),
                     "mrays_per_s": ((s.rays_primary + s.rays_secondary) / max(1, s.renders) / 1e6) / (r_val["stages"][k]["Ray Trace"] / 1e3)
@@ -809,7 +818,7 @@ def main():
             line["parity_crc_ok"] = bool(parity and parity["ranks_agree"] and parity["equals_single_gpu"])
             line["parity"] = parity
         if "pan" in extras:
-            line["pan"] = {"value": 40 / (ms_pan / 1e3), "unit": "frames/s", "frames": 40, "world_units_per_frame": PAN_STEP,
+            line["pan"] = {"value": args.steps / (ms_pan / 1e3), "unit": "frames/s", "frames": args.steps, "world_units_per_frame": PAN_STEP,
                            "gbuffer_ms_per_frame": extras["pan"]["gbuffer_ms_per_frame"], "stages_ms": extras["pan"]["stages"],
                            "note": "includes the G-buffer ray cast every frame (N > 1: hr_gbuffer_render_sharded, this rank's rows only)"}
         if k5_dense:

@@ -33,7 +33,7 @@
 #include <cfloat>
 
 #ifndef LEAF_MAX
-#define LEAF_MAX 2 // A/B (profiles/README.md, r2i): 2 beats 4 by 3 % on both the reflections and the shadows + AO workloads
+#define LEAF_MAX 2 // fewer triangle tests for a few more node steps than 4; chosen before the port, not re-measured on the H100
 #endif
 
 namespace {

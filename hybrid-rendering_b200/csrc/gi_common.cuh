@@ -145,7 +145,7 @@ __device__ __forceinline__ float2 texture_coord_fast(float3 dir, int probe_index
 
 // sample_irradiance, gi_common.glsl:188-320 (LINEAR_BLENDING undefined => sqrt-space blend).  A tolerance-checked colour
 // stage: reciprocal square roots / approximate reciprocals replace the IEEE sqrt + divide sequences (the IEEE forms made
-// K21 instruction-bound at 1.19 ms per 4K frame), the per-atlas constants are hoisted, and the probe loop is unrolled UNR
+// K21 instruction-bound), the per-atlas constants are hoisted, and the probe loop is unrolled UNR
 // times so the 8 atlas fetches of independent probes are in flight together.
 template <int UNR = 1>
 __device__ inline float3 sample_irradiance(const hr_ddgi_uniforms& d, const AtlasDev& at, float3 P, float3 N, float3 Wo)

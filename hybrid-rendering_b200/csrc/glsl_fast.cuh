@@ -20,6 +20,12 @@ __device__ __forceinline__ float4 h4_to_f4(uint2 w)
     return make_float4(a.x, a.y, b.x, b.y);
 }
 
+// Pixel-pair arithmetic of the a-trous kernels: one correctly rounded FFMA / FMUL / FADD per lane of the pair, never
+// contracted or reassociated, so both pixels get exactly what the scalar kernel computes.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
 // common.glsl:150-156
 __device__ __forceinline__ float3 octohedral_to_direction(float ex, float ey)
 {

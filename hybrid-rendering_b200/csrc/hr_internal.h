@@ -108,7 +108,7 @@ struct hr_ctx {
     // profiling
     bool         profiling = false;
     uint64_t     launches  = 0;
-    int          sm_count  = 148;
+    int          sm_count  = 132;
     cudaStream_t build_stream = nullptr;
     uint32_t*    d_brdf_lut = nullptr;  // 512 x 512 RG16F split-sum LUT (hr_brdf_lut_set); null: the IBL specular terms are 0
     unsigned long long* gbuf_ray_ctr = nullptr; // primary rays of hr_gbuffer_render (same slot layout as hr_pass::ray_ctr)

@@ -368,7 +368,7 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// K12, wavefront form (default).  ncu of the fused kernel above at 4K (profiles/r2a): 15.3 of 32 lanes active on average —
+// K12, wavefront form (hr_debug_set(7, 1)).  The fused kernel above has about half of its 32 lanes active on average —
 // glossy reflection rays of one 8x4 block take different paths through the BVH, and lanes that missed idle while their
 // neighbours shade and trace shadow rays.  Split in two:
 //   pass A  k_refl_trace: persistent warps pull 32x4-pixel jobs from an atomic counter, generate the reflection rays (sky and
@@ -755,14 +755,15 @@ void launch_ddgi_ray_trace(const hr_scene* sc, const hr_ddgi_uniforms& d, const 
 }
 
 // 0 (default) = fused kernel (one warp per 8x4 block: ray generation, closest hit, hit shading incl. its shadow ray);
-// 1 = wavefront (k_refl_trace + k_refl_shade).  Measured at 4K (profiles/r2c): fused 2.45 ms, wavefront 1.85 + 1.27 ms — the
-// refill keeps lanes supplied with rays, but lane-level divergence inside the while-while traversal (15.4 of 32 lanes active in
-// both forms) is what costs, and the 56 KB queue / stack footprint per CTA takes L1 away from the BVH (hit rate 40 % vs 64 %).
+// 1 = wavefront (k_refl_trace + k_refl_shade): 3.74 ms vs 2.63 per 4K frame (config 3, H100 SXM 80 GB, 700 W power limit) — the refill keeps lanes supplied with rays, but
+// lane-level divergence inside the while-while traversal (about half of the 32 lanes active in both forms) is what costs, and
+// the 56 KB queue / stack footprint per CTA takes L1 away from the BVH.
 // hr_debug_set key 7.
 int g_hr_refl_trace_impl = 0;
 // hr_debug_set key 10: resident 2-warp CTAs per SM the fused kernel's registers are tuned for (18 = 56 registers = default; 20 = 48;
-// 16 = 64; 14 = 72; 12 = 80).  Config 3 at 4K (profiles/README.md r2l / r2m): 12 -> 2.527 ms, 14 -> 2.366, 16 -> 2.208, 18 -> 2.133,
-// 20 -> 2.123 (172 bytes of spills): the kernel is latency-bound, resident warps buy more than registers.
+// 16 = 64; 14 = 72; 12 = 80).  Config 3 at 4K on an H100 SXM 80 GB (400 W power limit), K12 per frame: 12 -> 3.15 ms, 14 -> 3.00,
+// 16 -> 2.94, 18 -> 2.91, 20 -> 2.91: the kernel is latency-bound, resident warps buy more than registers (and than the spills
+// the smaller register budgets cost).
 int g_hr_refl_trace_minb = 18;
 
 void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
@@ -791,7 +792,7 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
         {
             cudaMalloc(&counter[dev], 64 * sizeof(unsigned int)); // one counter per stream slot would be needed for concurrent reflections passes; one pass per device here
             cudaFuncSetAttribute(k_refl_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            int sms = 148, per_sm = 1;
+            int sms = 132, per_sm = 1;
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_trace, RA_WARPS * 32, smem);
             ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);

@@ -186,14 +186,13 @@ void launch_tiled(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, 
 
 } // namespace
 
-// 0 = naive, 1 = tiled scalar kernel (64-105 us/iter at 4K).  hr_debug_set key 1.  (A sliding-register-window "chain" variant was
-// measured slower in round 1 — 72-107 us: its extra registers cost more occupancy than the saved shared-memory traffic bought —
-// and has been removed; profiles/README.md keeps the numbers.)
-// 3 = packed fp32x2 pixel-pair kernel (svgf_atrous_v3.cu; default: 53-85 us/iter, 47 % of HBM peak); it falls back to the
+// 0 = naive, 1 = tiled scalar kernel.  hr_debug_set key 1.  (A sliding-register-window "chain" variant, which traded
+// occupancy for shared-memory traffic, has been removed.)
+// 3 = pixel-pair kernel (svgf_atrous_v3.cu, default); it falls back to the
 // scalar tiled kernel for odd widths / phi_normal != 32.
 int g_hr_atrous_impl = 3;
 bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n, float sigma_z,
-                              float power, uint32_t* out, int row0, int row1, cudaStream_t st); // svgf_atrous_v3.cu (impl 3: packed fp32x2)
+                              float power, uint32_t* out, int row0, int row1, cudaStream_t st); // svgf_atrous_v3.cu (impl 3: pixel pairs)
 
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st)

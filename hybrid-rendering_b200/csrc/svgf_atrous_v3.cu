@@ -1,9 +1,9 @@
-// svgf_atrous_v3.cu — shadows a-trous (K4+K5, shadows_denoise_atrous.comp:94-174) with packed fp32x2 arithmetic.
+// svgf_atrous_v3.cu — shadows a-trous (K4+K5, shadows_denoise_atrous.comp:94-174) on pixel pairs.
 //
-// The scalar tiled kernel (svgf_atrous.cu) is instruction-issue bound (ncu r1b: 54 % issue-active, 13 % DRAM): ~23 FP32
-// instructions per tap.  Blackwell (sm_100) has packed two-wide fp32 instructions (FFMA2 / FMUL2 / FADD2, exposed as
-// __ffma2_rn / __fmul2_rn / __fadd2_rn): this kernel lets every thread filter TWO horizontally adjacent pixels and keeps
-// each per-pixel quantity of the pair in one 64-bit register pair, so one issue slot does the work for both pixels.
+// The scalar tiled kernel (svgf_atrous.cu) is instruction-issue bound: ~23 FP32 instructions per tap.  This kernel lets
+// every thread filter TWO horizontally adjacent pixels and keeps each per-pixel quantity of the pair in one 64-bit register
+// pair (gf::ffma2 / fmul2 / fadd2: two scalar instructions each on sm_90, which has no packed fp32), so the per-tap address
+// arithmetic, shared-memory loads and loop overhead are shared by both pixels.
 // Shared memory holds the staged tile as six fp32 planes (nx, ny, nz, z*log2e/sigma, visibility, variance); an aligned
 // LDS.64 fetches the same plane value for both pixels of a pair (taps at even column offsets), odd offsets (STEP = 1,
 // dx = +-1) use two LDS.32 straight into the register pair.  Out-of-image cells are staged with a zero normal (weight 0,
@@ -145,35 +145,35 @@ __global__ void __launch_bounds__(256) k_atrous_v3(GBufLevelDev g, const uint32_
                 PairCell    s;
                 s.nx = ld_pair(s_nx, si, aligned); s.ny = ld_pair(s_ny, si, aligned); s.nz = ld_pair(s_nz, si, aligned);
                 s.zs = ld_pair(s_zs, si, aligned); s.vis = ld_pair(s_vi, si, aligned); s.var = ld_pair(s_va, si, aligned);
-                const float2 dz = __ffma2_rn(s.zs, neg1, c.zs);
+                const float2 dz = ffma2(s.zs, neg1, c.zs);
                 float2       wZ;
                 wZ.x = fast_exp2(-fabsf(dz.x));
                 wZ.y = fast_exp2(-fabsf(dz.y));
-                const float2 dl = __ffma2_rn(s.vis, neg1, c.vis);
+                const float2 dl = ffma2(s.vis, neg1, c.vis);
                 float2       ea;
                 ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
                 ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-                ea   = __ffma2_rn(wZ, nl2e, ea);
+                ea   = ffma2(wZ, nl2e, ea);
                 float2 e;
                 e.x = fast_exp2(ea.x);
                 e.y = fast_exp2(ea.y);
-                float2 nd = __fmul2_rn(c.nz, s.nz);
-                nd        = __ffma2_rn(c.ny, s.ny, nd);
-                nd        = __ffma2_rn(c.nx, s.nx, nd);
+                float2 nd = fmul2(c.nz, s.nz);
+                nd        = ffma2(c.ny, s.ny, nd);
+                nd        = ffma2(c.nx, s.nx, nd);
                 nd.x      = fmaxf(nd.x, 0.0f);
                 nd.y      = fmaxf(nd.y, 0.0f);
-                float2 p = __fmul2_rn(nd, nd);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                const float2 wk = __fmul2_rn(e, p);
-                sumw = __fadd2_rn(sumw, wk);
-                s0   = __ffma2_rn(wk, s.vis, s0);
-                s1   = __ffma2_rn(__fmul2_rn(wk, wk), s.var, s1);
+                float2 p = fmul2(nd, nd);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                const float2 wk = fmul2(e, p);
+                sumw = fadd2(sumw, wk);
+                s0   = ffma2(wk, s.vis, s0);
+                s1   = ffma2(fmul2(wk, wk), s.var, s1);
             }
         const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-        float2       o0 = __fmul2_rn(s0, inv), o1 = __fmul2_rn(__fmul2_rn(s1, inv), inv);
+        float2       o0 = fmul2(s0, inv), o1 = fmul2(fmul2(s1, inv), inv);
         if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
         // sky pixels (linear z < 0) pass the input through
         const uint32_t r0 = c.zs.x < 0.0f ? f2_to_h2(c.vis.x, c.var.x) : f2_to_h2(o0.x, o1.x);
@@ -184,9 +184,8 @@ __global__ void __launch_bounds__(256) k_atrous_v3(GBufLevelDev g, const uint32_
 }
 
 // ---- row-interleaved tiles for the wide steps ---------------------------------------------------------------------------
-// With the dense 64x16 tile a step-8 iteration stages (64+16) x (16+16) texels for 1024 outputs (2.5x; 85 us vs 55 us for
-// step 1).  The taps of row y only touch rows y and y +- STEP, so a CTA that filters the 16 rows {Y0 + phase + STEP*j}
-// (one residue class of the row index) needs just 18 staged rows: (64+16) x 18 = 1.4x.  Rows stay contiguous in x, so
+// With the dense 64x16 tile a step-8 iteration stages (64+16) x (16+16) texels for 1024 outputs (2.5x).  The taps of row y
+// only touch rows y and y +- STEP, so a CTA that filters the 16 rows {Y0 + phase + STEP*j} (one residue class of the row index) needs just 18 staged rows: (64+16) x 18 = 1.4x.  Rows stay contiguous in x, so
 // global accesses are as coalesced as before.  compute_variance_center works at unit pixel spacing whatever the step:
 // the variance of the rows y-1 / y+1 (centre columns only) is staged into two extra single-plane buffers.
 template <int STEP>
@@ -296,35 +295,35 @@ __global__ void __launch_bounds__(256) k_atrous_v3s(GBufLevelDev g, const uint32
                 PairCell    s;
                 s.nx = ld_pair(s_nx, si, true); s.ny = ld_pair(s_ny, si, true); s.nz = ld_pair(s_nz, si, true);
                 s.zs = ld_pair(s_zs, si, true); s.vis = ld_pair(s_vi, si, true); s.var = ld_pair(s_va, si, true);
-                const float2 dz = __ffma2_rn(s.zs, neg1, c.zs);
+                const float2 dz = ffma2(s.zs, neg1, c.zs);
                 float2       wZ;
                 wZ.x = fast_exp2(-fabsf(dz.x));
                 wZ.y = fast_exp2(-fabsf(dz.y));
-                const float2 dl = __ffma2_rn(s.vis, neg1, c.vis);
+                const float2 dl = ffma2(s.vis, neg1, c.vis);
                 float2       ea;
                 ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
                 ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-                ea   = __ffma2_rn(wZ, nl2e, ea);
+                ea   = ffma2(wZ, nl2e, ea);
                 float2 e;
                 e.x = fast_exp2(ea.x);
                 e.y = fast_exp2(ea.y);
-                float2 nd = __fmul2_rn(c.nz, s.nz);
-                nd        = __ffma2_rn(c.ny, s.ny, nd);
-                nd        = __ffma2_rn(c.nx, s.nx, nd);
+                float2 nd = fmul2(c.nz, s.nz);
+                nd        = ffma2(c.ny, s.ny, nd);
+                nd        = ffma2(c.nx, s.nx, nd);
                 nd.x      = fmaxf(nd.x, 0.0f);
                 nd.y      = fmaxf(nd.y, 0.0f);
-                float2 p = __fmul2_rn(nd, nd);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                p        = __fmul2_rn(p, p);
-                const float2 wk = __fmul2_rn(e, p);
-                sumw = __fadd2_rn(sumw, wk);
-                s0   = __ffma2_rn(wk, s.vis, s0);
-                s1   = __ffma2_rn(__fmul2_rn(wk, wk), s.var, s1);
+                float2 p = fmul2(nd, nd);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                p        = fmul2(p, p);
+                const float2 wk = fmul2(e, p);
+                sumw = fadd2(sumw, wk);
+                s0   = ffma2(wk, s.vis, s0);
+                s1   = ffma2(fmul2(wk, wk), s.var, s1);
             }
         const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-        float2       o0 = __fmul2_rn(s0, inv), o1 = __fmul2_rn(__fmul2_rn(s1, inv), inv);
+        float2       o0 = fmul2(s0, inv), o1 = fmul2(fmul2(s1, inv), inv);
         if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
         const uint32_t r0 = c.zs.x < 0.0f ? f2_to_h2(c.vis.x, c.var.x) : f2_to_h2(o0.x, o1.x);
         const uint32_t r1 = c.zs.y < 0.0f ? f2_to_h2(c.vis.y, c.var.y) : f2_to_h2(o0.y, o1.y);
@@ -361,8 +360,8 @@ void launch_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, con
 } // namespace
 
 // 1 (default): step 8 uses the row-interleaved tiles (k_atrous_v3s); 2: steps 4 and 8; 0: dense tiles for every step
-// (hr_debug_set key 5).  Measured at 4K: step 8 dense 70.1 us -> interleaved 63.3 us; step 4 dense 55.5 us -> interleaved
-// 60.6 us (the two extra variance rows per filtered row cost more than the 8 halo rows they save).
+// (hr_debug_set key 5).  Config 2 (1080p) on an H100 SXM 80 GB, 700 W power limit: step 8 interleaved 25.1 us vs dense 25.9; step 4
+// interleaved 24.3 us vs dense 22.1 (the two extra variance rows per filtered row cost more than the 8 halo rows they save).
 int g_hr_atrous_rows = 1;
 
 // returns false when this variant does not support the configuration (caller falls back to the scalar kernels)

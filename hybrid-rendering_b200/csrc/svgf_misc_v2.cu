@@ -1,7 +1,6 @@
 // svgf_misc_v2.cu — shared-memory staged versions of the AO bilateral blur (K10) and the depth/normal-aware upsample
 // (K6 / K11 / K17).  The v1 kernels (svgf_misc.cu, svgf_reflections.cu) decode the octahedral normal and linearise the
-// depth of EVERY tap (9 resp. 4 per pixel, ~25 instructions each) and were instruction-issue bound (131 us upsample,
-// 2 x 63 us blur at 4K).  Here every G-buffer texel of the CTA's footprint is decoded once into shared memory.
+// depth of EVERY tap (9 resp. 4 per pixel, ~25 instructions each) and were instruction-issue bound.  Here every G-buffer texel of the CTA's footprint is decoded once into shared memory.
 //   K10 ao/ao_denoise_bilateral_blur.comp:75-139     K6 shadows_upsample.comp:62-109   K11 ao_upsample.comp:63-112
 //   K17 reflections_upsample.comp:62-109
 #include "glsl_fast.cuh"

@@ -1,10 +1,10 @@
-// svgf_refl_atrous_v2.cu — reflections a-trous (K15 + K16, reflections_denoise_atrous.comp:94-181) with packed fp32x2 arithmetic.
+// svgf_refl_atrous_v2.cu — reflections a-trous (K15 + K16, reflections_denoise_atrous.comp:94-181) on pixel pairs.
 //
 // This is the roofline kernel of BASELINE config 3 (4K full-res reflections: 36 algorithmic B/px/iteration, SURVEY.md §8d).  The
 // scalar kernel (svgf_reflections.cu::k_refl_atrous) is instruction-issue bound like its shadows twin was; this one applies the
 // same remedy as svgf_atrous_v3.cu: every thread filters TWO horizontally adjacent pixels and keeps each per-pixel quantity of
-// the pair in one 64-bit register pair, so the sm_100 packed instructions (FFMA2 / FMUL2 / FADD2) do the work of both pixels
-// in one issue slot.  Shared memory holds the staged tile + halo as nine fp32 planes (nx, ny, nz, z * log2e / sigma, r, g, b,
+// the pair in one 64-bit register pair (gf::ffma2 / fmul2 / fadd2), so addressing, shared-memory loads and loop overhead are
+// shared by both pixels.  Shared memory holds the staged tile + halo as nine fp32 planes (nx, ny, nz, z * log2e / sigma, r, g, b,
 // variance, luminance — the sample luminance is computed once per staged texel instead of once per tap); an aligned LDS.64
 // fetches a plane value for both pixels of a pair.  Out-of-image cells are staged with a zero normal (weight 0 = the
 // reference's `inside` test) and zero colour / variance (texelFetch robust-access zeros for compute_variance_center).
@@ -14,7 +14,7 @@
 #include <cuda.h> // CUtensorMap (driver types only; cuTensorMapEncodeTiled is fetched with cudaGetDriverEntryPoint)
 #include <vector>
 
-int g_hr_refl_atrous_minb = 4; // hr_debug_set key 8: registers tuned for 4 (default, measured: 110 us / iteration at 4K vs 141 us with 2), 3 or 2 CTAs per SM
+int g_hr_refl_atrous_minb = 4; // hr_debug_set key 8: registers tuned for 4 (default: resident CTAs hide the staging latency), 3 or 2 CTAs per SM
 
 namespace {
 
@@ -113,40 +113,40 @@ __device__ __forceinline__ void filter_pair(const float* __restrict__ s, int PL,
             const bool  al = ALIGNED_X || xx == 0;
             const float2 snx = ldp(s_nx, si, al), sny = ldp(s_ny, si, al), snz = ldp(s_nz, si, al), szs = ldp(s_zs, si, al);
             const float2 sr = ldp(s_r, si, al), sg = ldp(s_g, si, al), sb = ldp(s_b, si, al), sv = ldp(s_va, si, al), sl = ldp(s_lu, si, al);
-            const float2 dz = __ffma2_rn(szs, neg1, czs);
+            const float2 dz = ffma2(szs, neg1, czs);
             float2       wZ;
             wZ.x = fast_exp2(-fabsf(dz.x));
             wZ.y = fast_exp2(-fabsf(dz.y));
-            const float2 dl = __ffma2_rn(sl, neg1, clu);
+            const float2 dl = ffma2(sl, neg1, clu);
             float2       ea;
             ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
             ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-            ea   = __ffma2_rn(wZ, nl2e, ea);
+            ea   = ffma2(wZ, nl2e, ea);
             float2 e;
             e.x = fast_exp2(ea.x);
             e.y = fast_exp2(ea.y);
-            float2 nd = __fmul2_rn(cnz, snz);
-            nd        = __ffma2_rn(cny, sny, nd);
-            nd        = __ffma2_rn(cnx, snx, nd);
+            float2 nd = fmul2(cnz, snz);
+            nd        = ffma2(cny, sny, nd);
+            nd        = ffma2(cnx, snx, nd);
             nd.x      = fmaxf(nd.x, 0.0f);
             nd.y      = fmaxf(nd.y, 0.0f);
-            float2 p = __fmul2_rn(nd, nd);
-            p        = __fmul2_rn(p, p);
-            p        = __fmul2_rn(p, p);
-            p        = __fmul2_rn(p, p);
-            p        = __fmul2_rn(p, p);
-            const float2 wk = __fmul2_rn(e, p);
-            sumw = __fadd2_rn(sumw, wk);
-            ar   = __ffma2_rn(wk, sr, ar);
-            ag   = __ffma2_rn(wk, sg, ag);
-            ab   = __ffma2_rn(wk, sb, ab);
-            av   = __ffma2_rn(__fmul2_rn(wk, wk), sv, av);
+            float2 p = fmul2(nd, nd);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            const float2 wk = fmul2(e, p);
+            sumw = fadd2(sumw, wk);
+            ar   = ffma2(wk, sr, ar);
+            ag   = ffma2(wk, sg, ag);
+            ab   = ffma2(wk, sb, ab);
+            av   = ffma2(fmul2(wk, wk), sv, av);
         }
     const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-    o_r = __fmul2_rn(ar, inv);
-    o_g = __fmul2_rn(ag, inv);
-    o_b = __fmul2_rn(ab, inv);
-    o_v = __fmul2_rn(__fmul2_rn(av, inv), inv);
+    o_r = fmul2(ar, inv);
+    o_g = fmul2(ag, inv);
+    o_b = fmul2(ab, inv);
+    o_v = fmul2(fmul2(av, inv), inv);
 }
 
 // per-pixel class of the reference's early-outs (:119-128): 0 = sky -> 0, 1 = mirror / DDGI-rough -> pass-through, 2 = filter
@@ -367,9 +367,9 @@ void launch_r2s(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const
 // ---------------------------------------------------------------------------------------------------------------------------
 // TMA-staged, persistent form of the dense-tile kernel (steps 1, 2, 4).
 //
-// ncu of k_refl_atrous_v2 at 4K (profiles/r2c): 55 M warp instructions per iteration (the scalar kernel: 85 M) but only 34-45 %
-// issue-active — the top stall is long_scoreboard: every CTA first waits for its own staging loads from DRAM (L2 hit rate
-// 16-25 %: the images are larger than L2), and 2-4 resident CTAs per SM are not enough to cover that.  Here the loads leave the
+// k_refl_atrous_v2 issues far fewer instructions per iteration than the scalar kernel but stalls on long_scoreboard: every CTA
+// first waits for its own staging loads from DRAM (the images are larger than L2), and 2-4 resident CTAs per SM are not enough
+// to cover that.  Here the loads leave the
 // instruction stream: CTAs are persistent, tiles come from an atomic counter, and the three raw images of the NEXT tile (GB2, GB3,
 // input colour: tile + halo boxes of 8-byte texels) are fetched by the TMA engine (cp.async.bulk.tensor.2d, one elected
 // thread, completion on an mbarrier, out-of-image texels zero-filled by the hardware) while the CTA filters the CURRENT tile.
@@ -606,7 +606,7 @@ bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, co
     if (hr_once_per_device(configured))
     {
         cudaFuncSetAttribute(k_refl_atrous_tma<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM);
-        int sms = 148, per_sm = 1;
+        int sms = 132, per_sm = 1;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_atrous_tma<STEP>, 256, G::SMEM);
         ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);
@@ -621,11 +621,13 @@ bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, co
 
 } // namespace
 
-// hr_debug_set key 6: 0 = scalar kernel (svgf_reflections.cu), 1 = packed fp32x2 dense tiles for every step,
-// 2 = packed, row-interleaved tiles for steps >= 8, 3 (default) = 2 + TMA-staged persistent kernel for step 1,
+// hr_debug_set key 6: 0 = scalar kernel (svgf_reflections.cu), 1 = pixel-pair dense tiles for every step,
+// 2 = pixel pairs, row-interleaved tiles for steps >= 8, 3 (default) = 2 + TMA-staged persistent kernel for step 1,
 // 4 = 2 + TMA-staged persistent kernel for steps 1, 2 and 4.
-// Measured at 4K (profiles/r2e, us per iteration, steps 1 / 2 / 4): TMA 98 / 119 / 123, plain staging 108 / 101 / 122 — the TMA
-// kernel wins where its raw boxes + planes still allow 3 CTAs per SM (step 1: 74 KB) and loses where they allow 2 (82 / 104 KB).
+// Measured at 4K on an H100 SXM 80 GB (400 W power limit), us per iteration, steps 1 / 2 / 4 / 8: default 123 / 130 / 150 / 160,
+// 4 = 124 / 144 / 149 / 160, scalar kernel 165 / 166 / 178 / 234.  TMA staging loses at step 2, where its raw boxes + planes
+// allow only 2 CTAs per SM (82 KB), and wins at step 1 (74 KB, 3 CTAs per SM): on an H100 SXM 80 GB, 700 W power limit, step 1 takes
+// 113 us with TMA and 118 us with plain staging (2).
 int g_hr_refl_atrous_impl = 3;
 
 // returns false when this variant does not support the configuration (the caller falls back to the scalar kernel)

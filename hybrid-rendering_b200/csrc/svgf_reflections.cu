@@ -83,7 +83,7 @@ __device__ __forceinline__ uint32_t hist_ld32(const void* const* tab, const Hist
 // reference does 289 fetches per pixel): separable, each direction as a SLIDING window — stage the 48x24 rgb region; 144 threads
 // each walk half a staged row of one channel keeping the running 17-tap sums of c and c^2 (17 + 15 * 2 loads instead of
 // 16 * 17); 192 threads each walk one column of one of the six horizontal sums (17 + 7 * 2 loads instead of 8 * 17); every
-// pixel then reads its six window sums.  ncu (r2a) had this kernel at 1 733 instructions per pixel, 72 % issue-active.
+// pixel then reads its six window sums.
 // hp.img = last frame's temporal output (or prev_image), hp.aux = last frame's moments, of the rank that owns the row (PEER)
 template <bool PEER>
 __global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBufLevelDev prev, const uint2* __restrict__ input, const HistPeers hp, FrameConsts fc,

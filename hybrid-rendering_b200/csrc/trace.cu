@@ -427,11 +427,11 @@ __global__ void k_trace_closest(BvhDev bvh, const float* __restrict__ rays, size
 static inline dim3 mask_grid(int W, int mrow0, int mrow1) { return dim3(((W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, mrow1 - mrow0, 1); }
 
 // 0 = one warp per 8x4 block (default), 1 = persistent threads + ray compaction + LDS stack (hr_debug_set key 2).
-// Measured at 4K (profiles/README.md): shadows 585 us vs 712 us, AO 223 us vs 333 us — on this workload the 8x4 blocks are
-// almost uniformly active (coherent surfaces), so compaction buys little and the queue / refill bookkeeping costs more.
+// Config 2 (1080p) on an H100 SXM 80 GB, 700 W power limit: shadows K1 266 us vs 159, AO K7 144 us vs 77 — the 8x4 blocks are almost uniformly
+// active (coherent surfaces), so compaction buys little and the queue / refill bookkeeping costs more.
 int g_hr_trace_impl = 0;
 // hr_debug_set key 9: 1 = packet traversal for the shadow rays of K1 (single-GPU / band-local path), 0 (default) = per-lane traversal.
-// Measured on config 2 (1080p, profiles/README.md r2j): per-lane 147 us vs packet 332 us — the cone of a soft-shadow ray bundle makes
+// Config 2 (1080p) on an H100 SXM 80 GB, 700 W power limit: K1 with packets 352 us vs 159 per-lane — the cone of a soft-shadow ray bundle makes
 // the union of the lanes' paths much longer than any single path, and every lane tests every triangle of every visited leaf.
 int g_hr_shadow_packet = 0;
 
@@ -451,7 +451,7 @@ static void launch_pt(const GBufLevelDev& g, const BvhDev& bvh, const FrameConst
     {
         cudaMalloc(&counter[dev], sizeof(unsigned int));
         cudaFuncSetAttribute(k_ray_trace_mask_pt<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPtSmem);
-        int sms = 148, per_sm = 1;
+        int sms = 132, per_sm = 1;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_ray_trace_mask_pt<MODE>, PT_WARPS * 32, kPtSmem);
         ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);

@@ -44,7 +44,8 @@ __device__ __forceinline__ void count_rays(unsigned long long* ctr, int kind, ui
 }
 
 // ---- leaf triangles -------------------------------------------------------------------------------------------------
-// TRV_TRI_MODE (compile time, A/B'd on the GPU, profiles/README.md):
+// TRV_TRI_MODE (compile time A/B variants; mode 2 vs the default 0 on an H100 SXM 80 GB, 700 W power limit: config 3 K12 2.67 ms vs 2.63,
+// config 2 K1 169 us vs 159):
 //   0  three __ldg per triangle, issued where the compiler leaves them (it sinks v0 below the dt == 0 branch: two dependent
 //      memory round trips per triangle)
 //   1  all three 128-bit loads of a triangle issued up front (volatile asm: not sunk, not reordered)
@@ -109,17 +110,15 @@ __device__ __forceinline__ SlabSetup slab_setup(const Ray& r)
 __device__ __forceinline__ void node_test(const float4* __restrict__ nodes, int node, const SlabSetup& s, float tmin, float tmax, bool& h0, bool& h1,
                                           float& tn0, float& tn1, int& c0, int& c1)
 {
-    // The 64-byte node is fetched with two 256-bit loads (sm_100 LDG.E.256): the child indices travel with the z slabs, so
-    // they cannot be sunk below the box tests by the scheduler (a second L1 round trip per traversal step otherwise).
+    // The 64-byte node is fetched with four 128-bit loads issued back to back (volatile asm): the child indices are loaded
+    // up front, so the scheduler cannot sink them below the box tests (a second L1 round trip per traversal step otherwise).
     const float4* np = nodes + 4ull * node;
     float4        n0, n1, nz;
-    float         pad0, pad1;
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(n0.x), "=f"(n0.y), "=f"(n0.z), "=f"(n0.w), "=f"(n1.x), "=f"(n1.y), "=f"(n1.z), "=f"(n1.w)
-                 : "l"(np));
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8+32];"
-                 : "=f"(nz.x), "=f"(nz.y), "=f"(nz.z), "=f"(nz.w), "=r"(c0), "=r"(c1), "=f"(pad0), "=f"(pad1)
-                 : "l"(np));
+    int           pad0, pad1;
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(n0.x), "=f"(n0.y), "=f"(n0.z), "=f"(n0.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+16];" : "=f"(n1.x), "=f"(n1.y), "=f"(n1.z), "=f"(n1.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+32];" : "=f"(nz.x), "=f"(nz.y), "=f"(nz.z), "=f"(nz.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4+48];" : "=r"(c0), "=r"(c1), "=r"(pad0), "=r"(pad1) : "l"(np));
     float ax = fmaf(n0.x, s.idx, -s.ox), bx = fmaf(n0.y, s.idx, -s.ox);
     float ay = fmaf(n0.z, s.idy, -s.oy), by = fmaf(n0.w, s.idy, -s.oy);
     float az = fmaf(nz.x, s.idz, -s.oz), bz = fmaf(nz.y, s.idz, -s.oz);
@@ -136,7 +135,8 @@ __device__ __forceinline__ void node_test(const float4* __restrict__ nodes, int 
 
 // ---- 4-wide nodes (TRV_WIDE, compile time) -----------------------------------------------------------------------------
 // Per-lane traversal over bvh.wnodes (bvh_build.cu k_widen): one 112-byte fetch tests four boxes, so a ray makes about half
-// the DEPENDENT memory round trips of the binary walk (the kernels are bound by that latency chain, profiles/README.md).
+// the DEPENDENT memory round trips of the binary walk.  Slower than the binary walk on an H100 SXM 80 GB, 700 W power limit: config 3 K12
+// 2.88 ms vs 2.63, config 2 K1 168 us vs 159 — the kernels are not bound by that latency chain.
 // The hit entries are ordered near-to-far with a 5-exchange network on keys (entry distance bits | entry index; distances
 // are >= tmin >= 0, so their bit patterns order like unsigned integers), nearest child next, the others pushed far-to-near.
 #ifndef TRV_WIDE
@@ -150,12 +150,12 @@ __device__ __forceinline__ int wide_step(const float4* __restrict__ wnodes, int 
     const float4* np = wnodes + 8ull * node;
     float4        lx, hx, ly, hy, lz, hz;
     int           r0, r1, r2, r3;
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(lx.x), "=f"(lx.y), "=f"(lx.z), "=f"(lx.w), "=f"(hx.x), "=f"(hx.y), "=f"(hx.z), "=f"(hx.w) : "l"(np));
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8+32];"
-                 : "=f"(ly.x), "=f"(ly.y), "=f"(ly.z), "=f"(ly.w), "=f"(hy.x), "=f"(hy.y), "=f"(hy.z), "=f"(hy.w) : "l"(np));
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8+64];"
-                 : "=f"(lz.x), "=f"(lz.y), "=f"(lz.z), "=f"(lz.w), "=f"(hz.x), "=f"(hz.y), "=f"(hz.z), "=f"(hz.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(lx.x), "=f"(lx.y), "=f"(lx.z), "=f"(lx.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+16];" : "=f"(hx.x), "=f"(hx.y), "=f"(hx.z), "=f"(hx.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+32];" : "=f"(ly.x), "=f"(ly.y), "=f"(ly.z), "=f"(ly.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+48];" : "=f"(hy.x), "=f"(hy.y), "=f"(hy.z), "=f"(hy.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+64];" : "=f"(lz.x), "=f"(lz.y), "=f"(lz.z), "=f"(lz.w) : "l"(np));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4+80];" : "=f"(hz.x), "=f"(hz.y), "=f"(hz.z), "=f"(hz.w) : "l"(np));
     asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4+96];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "l"(np));
     uint32_t k0, k1, k2, k3;
 #define TRV_BOX(K, LX, HX, LY, HY, LZ, HZ)                                                              \

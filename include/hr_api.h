@@ -1,5 +1,5 @@
 /*
- * hr_api.h — C ABI of the B200-native ray-trace + SVGF hot path.
+ * hr_api.h — C ABI of the H100-native ray-trace + SVGF hot path.
  *
  * This is the drop-in boundary for the four render passes of diharaw/hybrid-rendering
  * (RayTracedShadows, RayTracedAO, RayTracedReflections, DDGI) and the stages either side of them

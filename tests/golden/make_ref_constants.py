@@ -4,18 +4,20 @@ write them to tests/golden/ref_constants.json.
 
 The reference (diharaw/hybrid-rendering) ships no tests, golden vectors or fixtures; the only reference-held data that
 can pin the oracle are the literals inside its shaders and headers.  This script parses them (nothing is typed in by
-hand) from /root/reference and records the file:line each value came from.  It runs in the build container only
-(/root/reference does not exist on the GPU box); the JSON is committed and tests/test_ref_constants.py checks the
-oracle (and, on the GPU, the CUDA kernels) against it.
+hand) from a checkout of the reference and records the file:line each value came from.  The reference is not part of
+this repository, so the JSON is committed and tests/test_ref_constants.py checks the oracle (and, on the GPU, the CUDA
+kernels) against it.
 
-    python tests/golden/make_ref_constants.py [/root/reference]
+    python tests/golden/make_ref_constants.py REFERENCE_CHECKOUT
 """
 import json
 import os
 import re
 import sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+if len(sys.argv) != 2:
+    sys.exit(__doc__)
+REF = sys.argv[1]
 SH = os.path.join(REF, "src", "shaders")
 SRC = os.path.join(REF, "src")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_constants.json")

@@ -1,6 +1,6 @@
 """bench.py contract on the CPU: the reference arm (`--impl reference`, the CPU oracle timed on the host cores) prints ONE JSON line
 with the keys the driver reads, for every BASELINE config, and — launched as N ranks — only rank 0 prints it.  The GPU arm needs
-a B200 and is exercised by the driver; its line carries the same keys plus roofline / clocks / gpu_launches."""
+an H100; its line carries the same keys plus roofline / clocks / gpu_launches."""
 import json
 import os
 import subprocess

@@ -2,8 +2,7 @@
 8-bit image of unoccluded-ray counts instead of the 1-bit mask, visibility = count / spp in the temporal stage.
 
 The CUDA kernels of this mode (k_ray_trace_count, k_temporal_count) mirror the validated 1-spp kernels; the ray counts must be
-exact against the oracle and the denoised images within the same tolerances as the 1-spp chains (confirmed on a B200 with the
-last GPU seconds of round 1: all three tests passed).
+exact against the oracle and the denoised images within the same tolerances as the 1-spp chains.
 """
 import numpy as np
 import pytest
