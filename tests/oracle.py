@@ -146,6 +146,15 @@ def zero_gbuf_mips(W, H, n_mips=3):
     return GBufMips(pyhr.GBufferHost(W, H), n_mips)
 
 
+def pass_size(W0, H0, scale):
+    """resolution of a pass at RayTraceScale `scale`: halved per level and clamped to 1 (hr_api.cu pass_common_create, the mip
+    chain of GBufMips), so that a 1-pixel dimension stays 1 rather than reaching 0"""
+    W, H = W0, H0
+    for _ in range(scale):
+        W, H = max(W // 2, 1), max(H // 2, 1)
+    return W, H
+
+
 def _coop_mask(o):
     """keep only the mask rows of this rank's ray-trace share, trash the rest, then let the exchange complete the image"""
     a, b = o.rt_share
@@ -159,9 +168,7 @@ def _coop_mask(o):
 class ShadowsOracle:
     def __init__(self, W0, H0, scale=0, spp=1):
         self.W0, self.H0, self.scale = W0, H0, scale
-        self.W, self.H = W0, H0
-        for _ in range(scale):
-            self.W, self.H = max(self.W // 2, 1), max(self.H // 2, 1)
+        self.W, self.H = pass_size(W0, H0, scale)
         W, H = self.W, self.H
         self.spp = spp  # > 1: SURVEY.md §8d definition (count image instead of the bit mask)
         self.count = np.zeros((H, W), np.uint8)
@@ -251,9 +258,7 @@ class ShadowsOracle:
 class AOOracle:
     def __init__(self, W0, H0, scale=1, spp=1):
         self.W0, self.H0, self.scale = W0, H0, scale
-        self.W, self.H = W0, H0
-        for _ in range(scale):
-            self.W, self.H = max(self.W // 2, 1), max(self.H // 2, 1)
+        self.W, self.H = pass_size(W0, H0, scale)
         W, H = self.W, self.H
         self.spp = spp
         self.count = np.zeros((H, W), np.uint8)
@@ -419,7 +424,8 @@ class DDGIOracle:
     """DDGI::render, src/ddgi.cpp:89-104"""
 
     def __init__(self, W0, H0, scale, params, bounds_min, bounds_max):
-        self.W, self.H, self.scale = W0 >> scale, H0 >> scale, scale
+        self.W, self.H = pass_size(W0, H0, scale)
+        self.scale = scale
         self.params = params
         self.u = ddgi_uniforms_from(params, bounds_min, bounds_max)
         u = self.u
@@ -455,7 +461,7 @@ class ReflectionsOracle:
 
     def __init__(self, W0, H0, scale, params):
         self.W0, self.H0, self.scale = W0, H0, scale
-        self.W, self.H = W0 >> scale, H0 >> scale
+        self.W, self.H = pass_size(W0, H0, scale)
         W, H = self.W, self.H
         self.params = params
         self.rt = np.zeros((H, W, 4), np.uint16)
