@@ -248,59 +248,6 @@ __global__ void k_pack_tiny(int n, const int* __restrict__ bounds, float4* __res
     out[3] = make_float4(__int_as_float(~((0 << 3) | (n - 1))), __int_as_float(~((0 << 3) | 0)), 0.0f, 0.0f);
 }
 
-// 4-wide nodes for the per-lane traversal (traverse.cuh wnode_test): the wide node of binary node i holds up to four
-// descendants of i — its two children, then twice the internal entry with the largest surface area replaced by ITS two
-// children (the SAH-greedy collapse of Wald et al. 2008).  One thread per binary node, no dependencies: wide node i is
-// written for EVERY i and a child reference keeps the binary index, so only the wide nodes reachable from the root are ever
-// read.  Halves the dependent node fetches per ray; hit results are unchanged (see the header: any topology gives the same hits).
-// Layout (8 x float4): lo.x[4] hi.x[4] lo.y[4] hi.y[4] lo.z[4] hi.z[4] ref[4] (as bits) pad.  Unused entries: a far degenerate
-// box (never hit) that refers to entry 0's child.
-__global__ void k_widen(int n_nodes, const float4* __restrict__ nodes, float4* __restrict__ out)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_nodes) return;
-    float lo[4][3], hi[4][3];
-    int   ref[4], cnt = 0;
-    auto  expand = [&](int node, int slot_a, int slot_b) {
-        const float4 n0 = nodes[4ull * node], n1 = nodes[4ull * node + 1], nz = nodes[4ull * node + 2], ch = nodes[4ull * node + 3];
-        lo[slot_a][0] = n0.x; hi[slot_a][0] = n0.y; lo[slot_a][1] = n0.z; hi[slot_a][1] = n0.w; lo[slot_a][2] = nz.x; hi[slot_a][2] = nz.y;
-        lo[slot_b][0] = n1.x; hi[slot_b][0] = n1.y; lo[slot_b][1] = n1.z; hi[slot_b][1] = n1.w; lo[slot_b][2] = nz.z; hi[slot_b][2] = nz.w;
-        ref[slot_a] = __float_as_int(ch.x);
-        ref[slot_b] = __float_as_int(ch.y);
-    };
-    expand(i, 0, 1);
-    cnt = 2;
-    for (int round = 0; round < 2; round++)
-    {
-        int   best = -1;
-        float best_area = -1.0f;
-        for (int k = 0; k < cnt; k++)
-        {
-            if (ref[k] < 0 || ref[k] >= n_nodes) continue; // leaf (or the tiny-scene dummy)
-            const float dx = hi[k][0] - lo[k][0], dy = hi[k][1] - lo[k][1], dz = hi[k][2] - lo[k][2];
-            const float area = dx * dy + dy * dz + dz * dx;
-            if (area > best_area) { best_area = area; best = k; }
-        }
-        if (best < 0) break;
-        expand(ref[best], best, cnt);
-        cnt++;
-    }
-    for (int k = cnt; k < 4; k++)
-    {
-        for (int a = 0; a < 3; a++) lo[k][a] = hi[k][a] = 1e30f;
-        ref[k] = ref[0];
-    }
-    float4* w = out + 8ull * i;
-    w[0] = make_float4(lo[0][0], lo[1][0], lo[2][0], lo[3][0]);
-    w[1] = make_float4(hi[0][0], hi[1][0], hi[2][0], hi[3][0]);
-    w[2] = make_float4(lo[0][1], lo[1][1], lo[2][1], lo[3][1]);
-    w[3] = make_float4(hi[0][1], hi[1][1], hi[2][1], hi[3][1]);
-    w[4] = make_float4(lo[0][2], lo[1][2], lo[2][2], lo[3][2]);
-    w[5] = make_float4(hi[0][2], hi[1][2], hi[2][2], hi[3][2]);
-    w[6] = make_float4(__int_as_float(ref[0]), __int_as_float(ref[1]), __int_as_float(ref[2]), __int_as_float(ref[3]));
-    w[7] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-}
-
 // Height of the binary tree: every leaf counts the edges to the root (both builders keep parent[], leaves at n-1+k, root -1).
 // The traversal stacks are sized for HR_BVH_MAX_DEPTH; hr_scene_build / hr_scene_rebuild refuse a deeper tree.
 __global__ void k_depth(int n, const int* __restrict__ parent, int* __restrict__ depth)
@@ -569,9 +516,8 @@ int hr_bvh_build(hr_scene* sc, cudaStream_t st)
         sc->n_nodes = 1;
         ctx->launches += 1;
     }
-    k_widen<<<(int)((sc->n_nodes + T - 1) / T), T, 0, st>>>((int)sc->n_nodes, sc->d_nodes, sc->d_wnodes);
     k_pack_tris<<<gb, T, 0, st>>>(sc->d_tri_verts, prim_order, n, sc->d_tris);
-    ctx->launches += 2;
+    ctx->launches += 1;
     HR_CHECK_LAUNCH(ctx);
     return HR_OK;
 }
@@ -581,7 +527,6 @@ BvhDev hr_bvh_view(const hr_scene* sc)
     BvhDev v;
     v.nodes         = sc->d_nodes;
     v.tris          = sc->d_tris;
-    v.wnodes        = sc->d_wnodes;
     v.root_is_valid = sc->n_tris > 0;
     return v;
 }

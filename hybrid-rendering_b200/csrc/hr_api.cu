@@ -11,15 +11,11 @@
 static std::string g_last_error;
 static std::mutex  g_err_mutex;
 extern int         g_hr_atrous_impl;
-extern int         g_hr_trace_impl;
 extern int         g_hr_bvh_quality;
 extern int         g_hr_force_shared_rt;
 extern int         g_hr_atrous_rows;
 extern int         g_hr_refl_atrous_impl;
-extern int         g_hr_refl_trace_impl;
 extern int         g_hr_refl_atrous_minb;
-extern int         g_hr_shadow_packet;
-extern int         g_hr_refl_trace_minb;
 extern int         g_hr_gather_impl;
 extern int         g_hr_force_peer_temporal;
 
@@ -169,15 +165,11 @@ const char* hr_last_error(hr_ctx* ctx)
 int hr_debug_set(int key, int value)
 {
     if (key == 1) { g_hr_atrous_impl = value; return HR_OK; }
-    if (key == 2) { g_hr_trace_impl = value; return HR_OK; }
     if (key == 3) { g_hr_bvh_quality = value; return HR_OK; }
     if (key == 4) { g_hr_force_shared_rt = value; return HR_OK; }
     if (key == 5) { g_hr_atrous_rows = value; return HR_OK; }
     if (key == 6) { g_hr_refl_atrous_impl = value; return HR_OK; }
-    if (key == 7) { g_hr_refl_trace_impl = value; return HR_OK; }
     if (key == 8) { g_hr_refl_atrous_minb = value; return HR_OK; }
-    if (key == 9) { g_hr_shadow_packet = value; return HR_OK; }
-    if (key == 10) { g_hr_refl_trace_minb = value; return HR_OK; }
     if (key == 11) { g_hr_gather_impl = value; return HR_OK; }
     if (key == 12) { g_hr_force_peer_temporal = value; return HR_OK; }
     return HR_ERR_INVALID_ARG;
@@ -290,7 +282,6 @@ int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, co
     ALLOC(sc->d_node_aabb, ni * 6 * sizeof(float));
     ALLOC(sc->d_flags, ni * sizeof(int));
     ALLOC(sc->d_nodes, ni * 4 * sizeof(float4));
-    ALLOC(sc->d_wnodes, ni * 8 * sizeof(float4));
     ALLOC(sc->d_depth, sizeof(int));
     ALLOC(sc->d_tris, n * 3 * sizeof(float4));
     if (n_materials && materials)
@@ -366,7 +357,7 @@ int hr_scene_destroy(hr_scene* sc)
     if (!sc) return HR_ERR_INVALID_ARG;
     if (sc->ctx && sc->ctx->scene == sc) sc->ctx->scene = nullptr;
     void* ptrs[] = { sc->d_tri_verts, sc->d_prim_inst, sc->d_prim_mat, sc->d_vnormals, sc->d_keys, sc->d_keys_sorted, sc->d_vals, sc->d_vals_sorted,
-                     sc->d_tri_aabb, sc->d_bounds_i, sc->d_children, sc->d_ranges, sc->d_parent, sc->d_node_aabb, sc->d_flags, sc->d_nodes, sc->d_wnodes, sc->d_depth, sc->d_tris,
+                     sc->d_tri_aabb, sc->d_bounds_i, sc->d_children, sc->d_ranges, sc->d_parent, sc->d_node_aabb, sc->d_flags, sc->d_nodes, sc->d_depth, sc->d_tris,
                      sc->d_materials, sc->d_sort_tmp, sc->d_ploc, sc->d_vuv, sc->d_vtb, sc->d_texels, sc->d_tex_desc, sc->d_mat_tex, sc->d_srgb_lut };
     for (void* p : ptrs) cudaFree(p);
     delete sc;

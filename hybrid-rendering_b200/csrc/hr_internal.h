@@ -38,7 +38,6 @@ struct GBufLevelDev {          // one mip of one G-buffer slot
 struct BvhDev {                // traversal view of hr_scene
     const float4* nodes;       // 4 x float4 per node (see bvh_build.cu)
     const float4* tris;        // 3 x float4 per triangle in leaf order: (v0,prim) (e1,0) (e2,0)
-    const float4* wnodes;      // 4-wide nodes, 8 x float4 each, indexed like `nodes` (bvh_build.cu k_widen); per-lane traversal
     int           root_is_valid;
 };
 
@@ -137,7 +136,6 @@ struct hr_scene {
     size_t    ploc_bytes = 0;
     // outputs
     float4*   d_nodes = nullptr;     // n_nodes*4
-    float4*   d_wnodes = nullptr;    // n_nodes*8: 4-wide nodes (k_widen)
     int*      d_depth = nullptr;     // height of the binary tree (k_depth)
     float4*   d_tris  = nullptr;     // n*3
     // shading data (reflections / ddgi hit shading)
@@ -198,7 +196,6 @@ struct hr_pass {
     uint2*    refl_rt = nullptr;
     uint2*    refl_rt_pp[2] = { nullptr, nullptr };   // ray-trace output by frame parity when the ranks trace cooperatively (refl_rt_pp[0] == refl_rt)
     unsigned int* work_counters = nullptr;             // tile / job counters of this pass's persistent kernels
-    float4*   refl_hits = nullptr;                     // wavefront K12: one hit record (t, primitive, u, v) per pixel
     uint2*    refl_temporal[2] = { nullptr, nullptr }; // current_output[pp] (also the history of the next frame)
     uint2*    refl_moments[2] = { nullptr, nullptr };
     uint2*    refl_prev = nullptr;                     // prev_image (blur_as_input)
@@ -259,7 +256,7 @@ void launch_ddgi_sample_probe_grid(const GBufLevelDev& g, const FrameConsts& fc,
                                    void* out, int row0, int row1, cudaStream_t st);
 void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
                                   float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
-                                  const uint8_t* sobol, const uint8_t* srk, void* out, void* hits, int row0, int row1, int chunk_first, int chunk_stride,
+                                  const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
                                   int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st); // chunk_stride > 1: only the 8-row chunks c = chunk_first + i * chunk_stride (rows are ignored)
 void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const void* input, const HistPeers& hist, const FrameConsts& fc, float alpha,
                                  float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);

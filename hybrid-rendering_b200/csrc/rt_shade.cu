@@ -296,6 +296,9 @@ struct ReflTraceParams { float bias, trim; int sample_gi, approximate_with_ddgi;
 // K12: warp = 8x4 pixel block (coherent reflection rays), 256 threads = 32x8 pixels
 // 2-warp CTAs (16x4 pixels): closest-hit rays + hit shading are heavy-tailed, small CTAs recycle their slots sooner (trace.cu)
 // MULTI = false: exactly the reference's one ray per pixel (straight-line code); true: the spp > 1 extension (sample loop)
+// MINB: resident 2-warp CTAs per SM the registers are tuned for; 18 (56 registers) for one ray per pixel.  Config 3 at 4K on an
+// H100 SXM 80 GB (400 W power limit), K12 per frame: 12 -> 3.15 ms, 14 -> 3.00, 16 -> 2.94, 18 -> 2.91, 20 -> 2.91: the kernel is
+// latency-bound, resident warps buy more than registers (and than the spills the smaller register budgets cost).
 template <bool MULTI, int MINB, bool TEX>
 __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev g, BvhDev bvh, ShadeDev sd, FrameConsts fc, hr_ddgi_uniforms d, gi::AtlasDev at,
                                                                 ReflTraceParams P, const uint8_t* __restrict__ sobol, const uint8_t* __restrict__ srk,
@@ -365,255 +368,6 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
     }
     const float inv_n = 1.0f / (float)n_s;
     out[idx] = pack_h4(acc.x * inv_n, acc.y * inv_n, acc.z * inv_n, ray_length);
-}
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// K12, wavefront form (hr_debug_set(7, 1)).  The fused kernel above has about half of its 32 lanes active on average —
-// glossy reflection rays of one 8x4 block take different paths through the BVH, and lanes that missed idle while their
-// neighbours shade and trace shadow rays.  Split in two:
-//   pass A  k_refl_trace: persistent warps pull 32x4-pixel jobs from an atomic counter, generate the reflection rays (sky and
-//           DDGI-rough pixels are finished right there), compact the rays that need tracing into a per-warp shared-memory
-//           queue, and traverse with all lanes busy: a lane whose ray terminates refills from the queue (closest hit, ties ->
-//           lowest primitive, so the result does not depend on the traversal order).  Node stack in shared memory.  Output:
-//           one 16-byte hit record per pixel (t, primitive, u, v).
-//   pass B  k_refl_shade: a CTA compacts the pixels of its 32x8 tile that hit something, so every lane shades a hit
-//           (surface fetch, direct light + its shadow ray, DDGI diffuse); misses get the sky colour.
-// Ray generation is a shared device function (pass B recomputes the ray direction instead of reading 16 more bytes).
-#define RA_WARPS 8
-#define RA_QUEUE 128
-#define RA_SM_STACK 24
-#define RA_REFILL_STEPS 8
-#define HIT_NO_RAY 0xFFFFFFFEu
-#define HIT_MISS 0xFFFFFFFFu
-
-enum { RG_SKY = 0, RG_DDGI = 1, RG_TRACE = 2 };
-
-// reflections_ray_trace.rgen:119-171 up to the traceRayEXT call: lobe selection and the reflection ray
-__device__ __forceinline__ int refl_ray_gen(const GBufLevelDev& g, const FrameConsts& fc, const ReflTraceParams& P, const uint8_t* __restrict__ sobol,
-                                            const uint8_t* __restrict__ srk, int x, int y, Ray& r, V3& Pw, V3& Wo, V3& N)
-{
-    const size_t idx   = (size_t)y * g.W + x;
-    const float  depth = __ldg(g.depth + idx);
-    if (depth == 1.0f) return RG_SKY;
-    const float  u = ((float)x + 0.5f) / (float)g.W, v = ((float)y + 0.5f) / (float)g.H;
-    const uint2  g2 = __ldg(g.gb2 + idx), g3 = __ldg(g.gb3 + idx);
-    const float2 e  = __half22float2(*reinterpret_cast<const __half2*>(&g2.x));
-    const float  roughness = __half22float2(*reinterpret_cast<const __half2*>(&g3.x)).x;
-    Pw = det::world_position_from_depth(u, v, depth, fc.view_proj_inverse);
-    N  = det::octohedral_to_direction(e.x, e.y);
-    Wo = det::normalize(det::sub(det::mk(fc.cam_pos[0], fc.cam_pos[1], fc.cam_pos[2]), Pw));
-    r.o    = det::add(Pw, det::scale(N, P.bias));
-    r.tmin = 0.001f;
-    r.tmax = 10000.0f;
-    if (roughness < 0.05f) { r.d = reflect(det::scale(Wo, -1.0f), N); return RG_TRACE; }
-    if (roughness > 0.75f && P.approximate_with_ddgi == 1) return RG_DDGI;
-    const float ex = det::sample_blue_noise(x, y, (int)fc.num_frames, 0, sobol, srk) * P.trim;
-    const float ey = det::sample_blue_noise(x, y, (int)fc.num_frames, 1, sobol, srk) * P.trim;
-    const V3    Wh = importance_sample_ggx(ex, ey, N, roughness);
-    r.d = reflect(det::scale(Wo, -1.0f), Wh);
-    return RG_TRACE;
-}
-
-struct QRayC { float ox, oy, oz; uint32_t pix; float dx, dy, dz, pad; };
-
-__global__ void __launch_bounds__(RA_WARPS * 32, 3) k_refl_trace(GBufLevelDev g, BvhDev bvh, FrameConsts fc, hr_ddgi_uniforms d, gi::AtlasDev at, ReflTraceParams P,
-                                                              const uint8_t* __restrict__ sobol, const uint8_t* __restrict__ srk, uint2* __restrict__ out,
-                                                              float4* __restrict__ hits, unsigned int* __restrict__ work_counter)
-{
-    extern __shared__ __align__(16) unsigned char ra_smem[];
-    QRayC(*s_queue)[RA_QUEUE]     = reinterpret_cast<QRayC(*)[RA_QUEUE]>(ra_smem);
-    int(*s_stack)[RA_WARPS * 32]  = reinterpret_cast<int(*)[RA_WARPS * 32]>(ra_smem + sizeof(QRayC) * RA_WARPS * RA_QUEUE);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
-    const int MW = (g.W + 7) >> 3, SBW = (MW + 3) >> 2;
-    const int mrow0 = P.row0 >> 2, mrow1 = (P.row1 + 3) >> 2;
-    const int n_chunks_mine = P.chunk_stride > 1 ? (((g.H + 7) >> 3) - P.chunk_first + P.chunk_stride - 1) / P.chunk_stride : 0;
-    const int n_sb = P.chunk_stride > 1 ? SBW * 2 * n_chunks_mine : SBW * (mrow1 - mrow0);
-    const uint32_t lt_mask = (1u << lane) - 1u;
-    QRayC* q = s_queue[warp];
-
-    for (;;)
-    {
-        int sb = 0;
-        if (lane == 0) sb = (int)atomicAdd(work_counter, 1u);
-        sb = __shfl_sync(0xFFFFFFFFu, sb, 0);
-        if (sb >= n_sb) break;
-        const int jr = sb / SBW, mx0 = (sb % SBW) * 4; // job row: a mask row (4 pixel rows) of the row range, or of this rank's chunk list
-        const int my = P.chunk_stride > 1 ? 2 * (P.chunk_first + (jr >> 1) * P.chunk_stride) + (jr & 1) : mrow0 + jr;
-        // ---- ray generation + compaction ----------------------------------------------------------------------------------
-        int count = 0;
-#pragma unroll 1
-        for (int w = 0; w < 4; w++)
-        {
-            const int x = (mx0 + w) * 8 + (lane & 7), y = my * 4 + (lane >> 3);
-            bool  need = false;
-            QRayC qr;
-            if (x < g.W && y < g.H && (P.chunk_stride > 1 || (y >= P.row0 && y < P.row1)))
-            {
-                const size_t idx = (size_t)y * g.W + x;
-                Ray r;
-                V3  Pw, Wo, N;
-                const int kind = refl_ray_gen(g, fc, P, sobol, srk, x, y, r, Pw, Wo, N);
-                if (kind == RG_TRACE)
-                {
-                    need  = true;
-                    qr.ox = r.o.x; qr.oy = r.o.y; qr.oz = r.o.z; qr.dx = r.d.x; qr.dy = r.d.y; qr.dz = r.d.z;
-                    qr.pix = (uint32_t)(w * 32 + lane);
-                    qr.pad = 0.0f;
-                }
-                else
-                {
-                    float3 color = make_float3(0.0f, 0.0f, 0.0f);
-                    if (kind == RG_DDGI)
-                    {
-                        using namespace gi;
-                        const V3 R = reflect(det::scale(Wo, -1.0f), N);
-                        color      = sample_irradiance(d, at, to_f3(Pw), to_f3(R), to_f3(Wo)) * P.rough_ddgi_intensity;
-                    }
-                    out[idx]  = pack_h4(fminf(color.x, 0.7f), fminf(color.y, 0.7f), fminf(color.z, 0.7f), -1.0f);
-                    hits[idx] = make_float4(0.0f, __uint_as_float(HIT_NO_RAY), 0.0f, 0.0f);
-                }
-            }
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, need);
-            if (need) q[count + __popc(b & lt_mask)] = qr;
-            count += __popc(b);
-        }
-        __syncwarp();
-        count_rays(fc.ray_ctr, 0, lane == 0 ? (uint32_t)count : 0u);
-        // ---- closest-hit traversal with dynamic refill ---------------------------------------------------------------------
-        int       head  = 0;
-        bool      valid = false;
-        Ray       ray;
-        SlabSetup ss;
-        int       node = SENTINEL, sp = 0, ovf[STACK_SIZE - RA_SM_STACK];
-        uint32_t  pix = 0, best_prim = HIT_MISS;
-        float     best_t = 0.0f, best_u = 0.0f, best_v = 0.0f;
-        ray.tmin = 0.001f;
-        ray.tmax = 10000.0f;
-        for (;;)
-        {
-            const uint32_t idle = __ballot_sync(0xFFFFFFFFu, !valid);
-            if (idle)
-            {
-                if (!valid)
-                {
-                    const int mine = head + __popc(idle & lt_mask);
-                    if (mine < count)
-                    {
-                        const QRayC r = q[mine];
-                        ray.o = det::mk(r.ox, r.oy, r.oz); ray.d = det::mk(r.dx, r.dy, r.dz);
-                        pix   = r.pix;
-                        ss    = slab_setup(ray);
-                        node  = 0;
-                        sp    = 0;
-                        best_t = ray.tmax; best_prim = HIT_MISS; best_u = best_v = 0.0f;
-                        valid = true;
-                    }
-                }
-                head += __popc(idle);
-            }
-            if (!__any_sync(0xFFFFFFFFu, valid)) break;
-#pragma unroll 1
-            for (int it = 0; it < RA_REFILL_STEPS; it++)
-            {
-                while (valid && node >= 0 && node != SENTINEL)
-                {
-                    bool  h0, h1;
-                    float t0, t1;
-                    int   c0, c1;
-                    node_test(bvh.nodes, node, ss, ray.tmin, best_t, h0, h1, t0, t1, c0, c1);
-                    if (!h0 && !h1)
-                    {
-                        if (sp == 0) node = SENTINEL;
-                        else { --sp; node = sp < RA_SM_STACK ? s_stack[sp][tid] : ovf[sp - RA_SM_STACK]; }
-                    }
-                    else
-                    {
-                        node = h0 ? c0 : c1;
-                        if (h0 && h1)
-                        {
-                            if (t1 < t0) { const int tmp = c1; c1 = node; node = tmp; }
-                            if (sp < RA_SM_STACK) s_stack[sp][tid] = c1;
-                            else if (sp < STACK_SIZE) ovf[sp - RA_SM_STACK] = c1;
-                            if (sp < STACK_SIZE) sp++;
-                        }
-                    }
-                }
-                if (valid && node < 0)
-                {
-                    const int leaf  = ~node;
-                    const int first = leaf >> 3, cnt = (leaf & 7) + 1;
-                    for (int k = 0; k < cnt; k++)
-                    {
-                        const float4 A = __ldg(bvh.tris + 3ull * (first + k));
-                        const float4 B = __ldg(bvh.tris + 3ull * (first + k) + 1);
-                        const float4 C = __ldg(bvh.tris + 3ull * (first + k) + 2);
-                        float        t, u, v;
-                        if (ray_triangle(A, B, C, ray, t, u, v))
-                        {
-                            const uint32_t prim = __float_as_uint(A.w);
-                            if (t < best_t || (t == best_t && prim < best_prim)) { best_t = t; best_prim = prim; best_u = u; best_v = v; }
-                        }
-                    }
-                    if (sp == 0) node = SENTINEL;
-                    else { --sp; node = sp < RA_SM_STACK ? s_stack[sp][tid] : ovf[sp - RA_SM_STACK]; }
-                }
-                if (valid && node == SENTINEL)
-                { // traversal finished: publish the hit record of this lane's pixel
-                    const int x = (mx0 + (int)(pix >> 5)) * 8 + (int)(pix & 7u), y = my * 4 + (int)((pix & 31u) >> 3);
-                    hits[(size_t)y * g.W + x] = make_float4(best_t, __uint_as_float(best_prim), best_u, best_v);
-                    valid = false;
-                }
-                if (__any_sync(0xFFFFFFFFu, !valid)) break; // somebody can refill (or everybody is done)
-            }
-        }
-        __syncwarp();
-    }
-}
-
-// pass B: 32x8-pixel tile per CTA, hit pixels compacted so that every lane shades
-__global__ void __launch_bounds__(256) k_refl_shade(GBufLevelDev g, BvhDev bvh, ShadeDev sd, FrameConsts fc, hr_ddgi_uniforms d, gi::AtlasDev at, ReflTraceParams P,
-                                                     const uint8_t* __restrict__ sobol, const uint8_t* __restrict__ srk, const float4* __restrict__ hits,
-                                                     uint2* __restrict__ out)
-{
-    __shared__ uint16_t s_list[256];
-    __shared__ int      s_warp_base[9];
-    const int    lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int    x0 = blockIdx.x * 32, y0 = P.chunk_stride > 1 ? 8 * (P.chunk_first + (int)blockIdx.y * P.chunk_stride) : P.row0 + blockIdx.y * 8;
-    const int    y_end = P.chunk_stride > 1 ? g.H : P.row1;
-    const float3 sky = make_float3(P.sky[0], P.sky[1], P.sky[2]);
-    {
-        const int x = x0 + lane, y = y0 + warp;
-        bool      is_hit = false;
-        if (x < g.W && y < g.H && y < y_end)
-        {
-            const size_t   idx  = (size_t)y * g.W + x;
-            const uint32_t prim = __float_as_uint(__ldg(reinterpret_cast<const float*>(hits + idx) + 1));
-            if (prim == HIT_MISS) out[idx] = pack_h4(fminf(sky.x, 0.7f), fminf(sky.y, 0.7f), fminf(sky.z, 0.7f), -1.0f); // rmiss: colour = sky, ray_length stays -1
-            else if (prim != HIT_NO_RAY) is_hit = true;
-        }
-        const uint32_t b = __ballot_sync(0xFFFFFFFFu, is_hit);
-        if (lane == 0) s_warp_base[warp + 1] = __popc(b);
-        __syncthreads();
-        if (threadIdx.x == 0)
-        {
-            s_warp_base[0] = 0;
-            for (int w = 1; w <= 8; w++) s_warp_base[w] += s_warp_base[w - 1];
-        }
-        __syncthreads();
-        if (is_hit) s_list[s_warp_base[warp] + __popc(b & ((1u << lane) - 1u))] = (uint16_t)threadIdx.x;
-        __syncthreads();
-    }
-    const int n_hits = s_warp_base[8];
-    if ((int)threadIdx.x >= n_hits) return;
-    const int    t   = s_list[threadIdx.x];
-    const int    x = x0 + (t & 31), y = y0 + (t >> 5);
-    const size_t idx = (size_t)y * g.W + x;
-    const float4 h   = __ldg(hits + idx);
-    Ray r;
-    V3  Pw, Wo, N;
-    refl_ray_gen(g, fc, P, sobol, srk, x, y, r, Pw, Wo, N);
-    const float3 color = shade_hit(bvh, sd, fc.light, r, __float_as_uint(h.y), h.z, h.w, false, 0.0f, 0.0f, sky, P.sample_gi == 1, d, at, P.gi_intensity, fc.ray_ctr, P.ibl);
-    out[idx] = pack_h4(fminf(color.x, 0.7f), fminf(color.y, 0.7f), fminf(color.z, 0.7f), 0.001f + h.x);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -754,21 +508,9 @@ void launch_ddgi_ray_trace(const hr_scene* sc, const hr_ddgi_uniforms& d, const 
     else k_ddgi_ray_trace<false><<<probe1 - probe0, threads, 0, st>>>(hr_bvh_view(sc), shade_view(sc), d, at, light, P, (uint2*)radiance, (uint2*)dirdepth, sc->tex);
 }
 
-// 0 (default) = fused kernel (one warp per 8x4 block: ray generation, closest hit, hit shading incl. its shadow ray);
-// 1 = wavefront (k_refl_trace + k_refl_shade): 3.74 ms vs 2.63 per 4K frame (config 3, H100 SXM 80 GB, 700 W power limit) — the refill keeps lanes supplied with rays, but
-// lane-level divergence inside the while-while traversal (about half of the 32 lanes active in both forms) is what costs, and
-// the 56 KB queue / stack footprint per CTA takes L1 away from the BVH.
-// hr_debug_set key 7.
-int g_hr_refl_trace_impl = 0;
-// hr_debug_set key 10: resident 2-warp CTAs per SM the fused kernel's registers are tuned for (18 = 56 registers = default; 20 = 48;
-// 16 = 64; 14 = 72; 12 = 80).  Config 3 at 4K on an H100 SXM 80 GB (400 W power limit), K12 per frame: 12 -> 3.15 ms, 14 -> 3.00,
-// 16 -> 2.94, 18 -> 2.91, 20 -> 2.91: the kernel is latency-bound, resident warps buy more than registers (and than the spills
-// the smaller register budgets cost).
-int g_hr_refl_trace_minb = 18;
-
 void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
                                   float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
-                                  const uint8_t* sobol, const uint8_t* srk, void* out, void* hits, int row0, int row1, int chunk_first, int chunk_stride,
+                                  const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
                                   int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st)
 {
     const int n_chunks_mine = chunk_stride > 1 ? (((g.H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0;
@@ -779,30 +521,7 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
     memset(&du, 0, sizeof(du));
     if (d) du = *d;
     gi::AtlasDev at { (const uint2*)irr, (const uint32_t*)depth };
-    const bool textured = sc->tex.n_textures > 0; // material textures: the TEX instantiations of the fused kernel (the wavefront variant has none)
-    if (g_hr_refl_trace_impl == 1 && hits && row0 % 4 == 0 && spp <= 1 && !textured) // spp > 1 runs on the fused kernel
-    {
-        static unsigned int* counter[64] = {};
-        static int           ctas[64]    = {};
-        const size_t smem = sizeof(QRayC) * RA_WARPS * RA_QUEUE + sizeof(int) * RA_SM_STACK * RA_WARPS * 32;
-        int dev = 0;
-        cudaGetDevice(&dev);
-        dev &= 63;
-        if (!counter[dev])
-        {
-            cudaMalloc(&counter[dev], 64 * sizeof(unsigned int)); // one counter per stream slot would be needed for concurrent reflections passes; one pass per device here
-            cudaFuncSetAttribute(k_refl_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            int sms = 132, per_sm = 1;
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_trace, RA_WARPS * 32, smem);
-            ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);
-        }
-        cudaMemsetAsync(counter[dev], 0, sizeof(unsigned int), st);
-        k_refl_trace<<<ctas[dev], RA_WARPS * 32, smem, st>>>(g, hr_bvh_view(sc), fc, du, at, P, sobol, srk, (uint2*)out, (float4*)hits, counter[dev]);
-        dim3 gridb((g.W + 31) / 32, chunk_stride > 1 ? n_chunks_mine : (row1 - row0 + 7) / 8);
-        k_refl_shade<<<gridb, 256, 0, st>>>(g, hr_bvh_view(sc), shade_view(sc), fc, du, at, P, sobol, srk, (const float4*)hits, (uint2*)out);
-        return;
-    }
+    const bool textured = sc->tex.n_textures > 0; // material textures: the TEX instantiations
     dim3 grid((g.W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
     const tex::TexDev& T = sc->tex;
 #define HR_K12_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, du, at, P, sobol, srk, (uint2*)out, T
@@ -812,10 +531,6 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
         else k_reflections_ray_trace<false, 18, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
     }
     else if (spp > 1) k_reflections_ray_trace<true, 8, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else if (g_hr_refl_trace_minb == 14) k_reflections_ray_trace<false, 14, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else if (g_hr_refl_trace_minb == 12) k_reflections_ray_trace<false, 12, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else if (g_hr_refl_trace_minb == 16) k_reflections_ray_trace<false, 16, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else if (g_hr_refl_trace_minb == 20) k_reflections_ray_trace<false, 20, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
     else k_reflections_ray_trace<false, 18, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
 #undef HR_K12_ARGS
 }

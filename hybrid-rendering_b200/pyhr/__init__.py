@@ -10,7 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 PKG_ROOT = os.path.dirname(_HERE)
-BUILD_DIR = os.path.join(PKG_ROOT, os.environ.get("HR_BUILD_DIR", "build"))  # HR_BUILD_DIR: A/B of compile-time kernel variants (Makefile VARIANT=)
+BUILD_DIR = os.path.join(PKG_ROOT, "build")
 LIB_PRODUCT = os.path.join(BUILD_DIR, "libhr_b200.so")
 LIB_SYNTH = os.path.join(BUILD_DIR, "libhr_synth.so")
 

@@ -511,14 +511,11 @@ HR_API int hr_pass_destroy(hr_pass* pass);
 HR_API int hr_ctx_set_profiling(hr_ctx* ctx, int enabled);
 HR_API int hr_pass_stage_times(hr_pass* pass, const char** names, float* ms, int cap, int* n);
 /* Test / A-B hook.  key 1 = a-trous implementation (0 naive global-memory kernel, 1 shared-memory tiled kernel,
- * 3 packed fp32x2 pixel-pair kernel = default); key 2 = traversal kernel (0 one warp per 8x4 block = default, 1 persistent
- * threads + ray compaction); key 3 = BVH topology used by the next hr_scene_build / hr_scene_rebuild (0 Karras radix tree,
+ * 3 packed fp32x2 pixel-pair kernel = default); key 3 = BVH topology used by the next hr_scene_build / hr_scene_rebuild (0 Karras radix tree,
  * 1 PLOC agglomerative clustering = default); key 4 = run the cooperative (multi-GPU) ray-trace kernel on a single GPU;
  * key 5 = a-trous row-interleaved tiles: 1 = step 8 only (default), 2 = steps 4 and 8, 0 = dense tiles for every step; key 6 = reflections
  * a-trous (0 scalar kernel, 1 packed fp32x2 dense tiles, 2 = packed + row-interleaved tiles for steps >= 8, 3 = 2 + TMA-staged
- * persistent kernel for step 1 = default, 4 = TMA for steps 1, 2, 4); key 7 = reflections ray trace (0 fused kernel = default, 1 wavefront:
- * persistent closest-hit traversal with ray refill + compacted hit shading); key 8 = reflections a-trous register tuning (CTAs / SM);
- * key 9 = shadow rays of K1: 0 per-lane traversal = default, 1 packet traversal; key 10 = fused reflections ray trace register tuning (CTAs / SM);
+ * persistent kernel for step 1 = default, 4 = TMA for steps 1, 2, 4); key 8 = reflections a-trous register tuning (CTAs / SM);
  * key 11 = final-output gather: 1 point-to-point = default, 0 per-band broadcasts; key 12 = run the peer-history K14 on one GPU (overhead A/B).  None of them changes a result bit
  * of the visibility masks; keys 1 and 5 select kernels whose outputs agree to the last fp16 bit on the test scenes. */
 HR_API int hr_debug_set(int key, int value);

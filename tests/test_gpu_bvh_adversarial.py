@@ -3,16 +3,9 @@
 The bit-exact claim of every ray-traced pass rests on the box test being conservative: whatever the tree, a box that holds a
 triangle the ray hits in (t_min, t_max) must be entered.  These tests check that claim directly with hr_trace_any /
 hr_trace_closest (any flag, t, primitive and barycentrics compared bit for bit) under both tree builders, through the
-packet walk of the G-buffer producer and the shadows / AO ray-trace kernels, and in the compile-time traversal variants
-(4-wide nodes, next-triangle prefetch), each in a child process on its own build.
+packet walk of the G-buffer producer and through the shadows / AO ray-trace kernels.
 """
 import ctypes as C
-import json
-import os
-import shutil
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -142,7 +135,7 @@ class switches:
 
     def __init__(self, lib, **kv):
         self.lib, self.kv = lib, {int(k[1:]): v for k, v in kv.items()}
-        self.defaults = {2: 0, 3: 1, 7: 0, 9: 0}
+        self.defaults = {3: 1}
 
     def __enter__(self):
         for k, v in self.kv.items():
@@ -239,8 +232,7 @@ def with_roof(tri):
 @pytest.mark.parametrize("case", sorted(PASS_CASES))
 def test_gbuffer_shadows_ao_walks_match_the_oracle(case):
     """hr_gbuffer_render (packet closest-hit walk) bit for bit against orc_gbuffer, then the shadows and AO visibility masks
-    against the oracle with the default per-lane kernels, packet shadow rays (hr_debug_set(9, 1)) and the persistent-thread
-    kernels (hr_debug_set(2, 1)), under both tree builders"""
+    (per-lane walk) against the oracle, under both tree builders"""
     scene, rel = PASS_CASES[case]
     tri = with_roof(B.SCENES[scene]())
     lo, hi = B.scene_bounds(tri)
@@ -274,82 +266,19 @@ def test_gbuffer_shadows_ao_walks_match_the_oracle(case):
                 osh.render(ss.scene, cur, O.zero_gbuf_mips(GB_W, GB_H), f, bn)
                 oao.render(ss.scene, cur, O.zero_gbuf_mips(GB_W, GB_H), f, bn)
                 ctx.gbuffer_upload(f.ping_pong, ref)
-                for mode, sw in (("per-lane", {}), ("packet", {"k9": 1}), ("persistent", {"k2": 1})):
-                    with switches(ctx.lib, **sw):
-                        sh, ao = pyhr.Pass(ctx, "shadows", GB_W, GB_H, 0), pyhr.Pass(ctx, "ao", GB_W, GB_H, 0)
-                        try:
-                            sh.render(f)
-                            ao.render(f)
-                            if not np.array_equal(sh.download(0), osh.mask):
-                                failures.append(f"{topology} / {mode}: shadow mask")
-                            if not np.array_equal(ao.download(0), oao.mask):
-                                failures.append(f"{topology} / {mode}: AO mask")
-                        finally:
-                            sh.destroy()
-                            ao.destroy()
+                sh, ao = pyhr.Pass(ctx, "shadows", GB_W, GB_H, 0), pyhr.Pass(ctx, "ao", GB_W, GB_H, 0)
+                try:
+                    sh.render(f)
+                    ao.render(f)
+                    if not np.array_equal(sh.download(0), osh.mask):
+                        failures.append(f"{topology}: shadow mask")
+                    if not np.array_equal(ao.download(0), oao.mask):
+                        failures.append(f"{topology}: AO mask")
+                finally:
+                    sh.destroy()
+                    ao.destroy()
             finally:
                 ctx.lib.hr_scene_destroy(h)
         assert not failures, f"{case}: {failures}"
     finally:
         ctx.close()
-
-
-# ---------------------------------------------------------------------------------------------- compile-time variants
-VARIANTS = {"wide": "-DTRV_WIDE=1", "tri_prefetch": "-DTRV_TRI_MODE=2"}
-TRAVERSAL_OBJS = ("trace.o", "rt_shade.o", "gbuffer.o")  # the objects that include traverse.cuh
-
-
-@pytest.fixture(scope="session")
-def variant_builds(tmp_path_factory):
-    """one library per variant in a temporary directory: the objects that do not include traverse.cuh are copied from the
-    default build (with their times, so make keeps them) and the three that do are compiled with the variant's flags"""
-    pkg = os.path.dirname(os.path.dirname(os.path.abspath(pyhr.__file__)))
-    default = pyhr.BUILD_DIR
-    out = {}
-    for name, flags in VARIANTS.items():
-        d = str(tmp_path_factory.mktemp(f"build_{name}"))
-        for fn in os.listdir(default):
-            if fn.endswith(".o") and fn not in TRAVERSAL_OBJS or fn == "libhr_synth.so":
-                shutil.copy2(os.path.join(default, fn), os.path.join(d, fn))
-        r = subprocess.run(["make", "-j4", f"BUILD={d}", f"VARIANT={flags}", f"{d}/libhr_b200.so"], cwd=pkg, stdout=subprocess.PIPE,
-                           stderr=subprocess.STDOUT, text=True, timeout=1200)
-        assert r.returncode == 0, r.stdout[-3000:]
-        out[name] = d
-    return out
-
-
-def _child_main():
-    """run in a child process with HR_BUILD_DIR set: every scene x topology through hr_trace_*, JSON report on stdout"""
-    ctx = pyhr.Context(0)
-    res = {}
-    try:
-        for scene in sorted(B.SCENES):
-            for topology in sorted(TOPOLOGIES):
-                with switches(ctx.lib, k3=TOPOLOGIES[topology]):
-                    report, hits = check_scene(ctx, B.SCENES[scene](), n=1500)
-                res[f"{scene}/{topology}"] = {"hits": hits, "bad": bad_entries(report)}
-        with switches(ctx.lib, k3=1):
-            rc, h, _ = build(ctx, B.chain(B.MAX_DEPTH + 1))
-            ctx.check(rc, "hr_scene_build")
-            ctx.check(ctx.lib.hr_scene_set_current(ctx.h, h), "hr_scene_set_current")
-            rays, x = chain_rays(B.MAX_DEPTH + 1)
-            _, t, p, _ = gpu_trace(ctx, rays)
-            res["chain"] = {"hits": len(rays), "bad": {} if np.array_equal(p, np.arange(len(rays))) and np.array_equal(t, x) else {"chain": [1, 1]}}
-            ctx.lib.hr_scene_destroy(h)
-    finally:
-        ctx.close()
-    print(json.dumps(res))
-
-
-@pytest.mark.parametrize("variant", sorted(VARIANTS))
-def test_traversal_variant_matches_bruteforce(variant_builds, variant):
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, HR_BUILD_DIR=variant_builds[variant])
-    env["PYTHONPATH"] = os.pathsep.join([here, os.path.dirname(os.path.abspath(pyhr.__file__)).rsplit(os.sep, 1)[0], env.get("PYTHONPATH", "")])
-    r = subprocess.run([sys.executable, "-c", "import test_gpu_bvh_adversarial as T; T._child_main()"], cwd=here, env=env,
-                       stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, timeout=1800)
-    assert r.returncode == 0, r.stderr[-3000:]
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    assert all(v["hits"] > 0 for v in res.values())
-    bad = {k: v["bad"] for k, v in res.items() if v["bad"]}
-    assert not bad, f"{variant}: rays that differ from brute force (any, closest): {bad}"

@@ -1,6 +1,4 @@
-"""Non-default traversal / BVH variants must produce the same bit-exact visibility masks as the oracle:
-  * hr_debug_set(2, 1): persistent-threads traversal kernel (warp ray compaction + shared-memory stack) — not the default
-    (the plain one-warp-per-8x4-block kernel is faster on coherent primary-surface rays) but a supported variant;
+"""The non-default BVH builder must produce the same bit-exact visibility masks as the oracle:
   * hr_debug_set(3, 0): Karras radix-tree topology instead of the default PLOC agglomerative build (hit results must not
     depend on the BVH topology)."""
 import numpy as np
@@ -12,10 +10,10 @@ import pyhr
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("dbg_key,dbg_val,dbg_default", [(2, 1, 0), (3, 0, 1)], ids=["persistent-traversal", "lbvh-topology"])
+@pytest.mark.parametrize("dbg_key,dbg_val,dbg_default", [(3, 0, 1)], ids=["lbvh-topology"])
 @pytest.mark.parametrize("scene_kind,tris,W,H,cam", [
     (pyhr.SCENE_SHADOWS_TEST, 0, 256, 144, ((0.0, 14.0, 34.0), (0.0, 3.0, 0.0))),
-    (pyhr.SCENE_ARCADE, 30000, 200, 104, ((0.0, 9.0, -4.0), (2.0, 7.0, 60.0))),  # width not a multiple of 32: partial super-blocks
+    (pyhr.SCENE_ARCADE, 30000, 200, 104, ((0.0, 9.0, -4.0), (2.0, 7.0, 60.0))),  # width not a multiple of 16: a partial last CTA
 ])
 def test_variant_masks_bit_exact(scene_kind, tris, W, H, cam, dbg_key, dbg_val, dbg_default):
     sc = pyhr.SynthScene(scene_kind, tris)
