@@ -216,6 +216,7 @@ struct hr_pass {
     uint2*    deferred_out = nullptr;                  // deferred shading combine: RGBA16F (Lo, 1)
     uint2*    post_img[2] = { nullptr, nullptr };      // TAA: m_image[2] (temporal_aa.cpp:196-212); path tracer: images[2]; [0] = tone map RGBA8
     uint32_t* pt_prim = nullptr;                       // path tracer: primitive hit by the last frame's primary ray (0xFFFFFFFF = sky)
+    uint32_t* pt_hash = nullptr;                       // path tracer, trace_indirect = 1: hash of the last frame's path (HR_PATH_TRACER_OUT_PATH_HASH)
     uint32_t  pt_frame_idx = 0;                        // GroundTruthPathTracer::m_frame_idx
     int       pt_ping_pong = 0;                        // GroundTruthPathTracer::m_ping_pong
     std::vector<void*> ddgi_grid_allocs;
@@ -321,7 +322,7 @@ void launch_deferred(const GBufLevelDev& g, const FrameConsts& fc, const void* s
                      const float* env3, const void* brdf_lut, void* out, int row0, int row1, cudaStream_t st); // deferred.cu
 // rt_shade.cu: ground-truth path tracer
 void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       const void* prev, void* out, uint32_t* out_prim, unsigned long long* ray_ctr, cudaStream_t st);
+                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, cudaStream_t st);
 // post.cu
 void launch_taa(const GBufLevelDev& g, const void* current, int current_channels, const void* history, const float* jitter_xy, float feedback_min, float feedback_max,
                 int sharpen, void* out, cudaStream_t st);

@@ -376,8 +376,9 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
 // RAY_THROUGHPUT + SAMPLE_SKY_LIGHT (rchit:13-16): the punctual light sampled on its disk with its shadow ray, one cosine-lobe sky sample
 // with its shadow ray; miss -> the sky colour; running average into an RGBA16F image.  As written in the reference the indirect bounce's
 // traceRayEXT is commented out (rchit:92-104) and indirect_lighting returns p_IndirectPayload.L = vec3(0): the image converges to direct +
-// sky lighting; max_ray_bounces only gates that dead branch.  The primary ray, the hit and the two shadow rays follow the deterministic chain
-// (det_math.cuh): hit primitive and binary visibilities equal the oracle's (oracle/orc_path_trace.cpp) exactly, colours within tolerance.
+// sky lighting; max_ray_bounces only gates that dead branch.  trace_indirect = 1 (DESIGN.md §7) traces the bounces up to max_ray_bounces
+// vertices.  The primary ray, the hit, the two shadow rays and the bounces follow the deterministic chain (det_math.cuh): hit primitives,
+// paths and binary visibilities equal the oracle's (oracle/orc_path_trace.cpp, orc_path_trace_indirect.cpp) exactly, colours within tolerance.
 struct PathTraceParams {
     float    view_inverse[16], proj_inverse[16];
     hr_light light;
@@ -394,10 +395,87 @@ __device__ __forceinline__ float4 mat_vec4(const float* M, float x, float y, flo
                        ((M[2] * x + M[6] * y) + M[10] * z) + M[14] * w, ((M[3] * x + M[7] * y) + M[11] * z) + M[15] * w);
 }
 
+// direct_lighting, lighting.glsl:117-196 with SOFT_SHADOWS and SAMPLE_SKY_LIGHT at one path vertex (rchit:112-141): draws the light's disk
+// sample, then the sky sample (two next_vec2), traces their shadow rays; the throughput (RAY_THROUGHPUT) is applied by the caller
+__device__ __forceinline__ float3 path_direct_lighting(const BvhDev& bvh, const PathTraceParams& P, const Surface& s, float roughness, V3 Wo, float3 F0, float3 cd,
+                                                       float3 sky, gi::RNG& rng)
+{
+    using namespace gi;
+    const float r1x = next_float(rng), r1y = next_float(rng); // next_vec2: the light's disk sample
+    const float r2x = next_float(rng), r2y = next_float(rng); // next_vec2: the sky sample
+    float3 Lo = f3(0, 0, 0);
+    Ray    sr;
+    sr.o    = det::add(s.P, det::scale(s.N, 0.1f));
+    sr.tmin = 0.01f;
+    {
+        const hr_light& light = P.light;
+        const float3    Li = make_float3(light.data2[0] * light.data0[3], light.data2[1] * light.data0[3], light.data2[2] * light.data0[3]);
+        V3    Wi;
+        float t_max, att;
+        det::fetch_light_properties_shadow(light, s.P, s.N, r1x, r1y, Wi, t_max, att);
+        const V3 Wh = det::normalize(det::add(Wo, Wi));
+        if (att > 0.0f)
+        {
+            sr.d    = Wi;
+            sr.tmax = t_max;
+            count_rays(P.ray_ctr, 1, 1u);
+            att *= trace_any(bvh, sr) ? 0.0f : 1.0f;
+        }
+        Lo = Lo + (evaluate_uber_brdf(cd, roughness, s.N, F0, Wo, Wh, Wi) * att) * Li;
+    }
+    {
+        const V3 Wi = det::sample_cosine_lobe(s.N, r2x, r2y);
+        const V3 Wh = det::normalize(det::add(Wo, Wi));
+        sr.d    = Wi;
+        sr.tmax = 10000.0f;
+        count_rays(P.ray_ctr, 1, 1u);
+        const float vis = trace_any(bvh, sr) ? 0.0f : 1.0f;
+        Lo = Lo + evaluate_uber_brdf(cd, roughness, s.N, F0, Wo, Wh, Wi) * (sky * vis);
+    }
+    return Lo;
+}
+
+// path-hash end codes (HR_PATH_TRACER_OUT_PATH_HASH)
+constexpr uint32_t PT_END_MISS = 0xFFFFFFFFu, PT_END_HORIZON = 0xFFFFFFFEu, PT_END_MAX_BOUNCES = 0xFFFFFFFDu;
+__device__ __forceinline__ uint32_t fnv1a(uint32_t h, uint32_t w) { return (h ^ w) * 16777619u; }
+
+// One sampled continuation at a path vertex (trace_indirect = 1, DESIGN.md §7).  Lobe choice, direction and horizon tests are geometry
+// (det_math.cuh); the throughput factor is (as-written lobe value) * N.Wi / (lobe probability * sampler pdf), evaluated without a closed-form
+// simplification because D_ggx's 1e-4 denominator clamp is active near the highlight.  false: the path ends (below the horizon, or a
+// specular sample whose pdf is not positive, e.g. roughness 0 where the as-written D_ggx is 0 everywhere).
+__device__ __forceinline__ bool sample_bounce(V3 N, V3 Wo, float3 F0, float3 cd, float roughness, float metallic, float u, float e1, float e2, V3& Wi, float3& weight)
+{
+    using namespace gi;
+    const float p_spec = 0.5f + 0.5f * det::clampf(metallic, 0.0f, 1.0f);
+    const bool  spec   = u < p_spec;
+    Wi = spec ? reflect(det::scale(Wo, -1.0f), importance_sample_ggx(e1, e2, N, roughness)) : det::sample_cosine_lobe(N, e1, e2);
+    if (det::dot(N, Wi) <= 0.0f || det::dot(N, Wo) <= 0.0f) return false;
+    const V3     Wh    = det::normalize(det::add(Wo, Wi));
+    const float  NdotL = fmaxf(det::dot(N, Wi), 0.0f), NdotV = fmaxf(det::dot(N, Wo), 0.0f), NdotH = fmaxf(det::dot(N, Wh), 0.0f), VdotH = fmaxf(det::dot(Wi, Wh), 0.0f);
+    const float  p5    = powf(1.0f - VdotH, 5.0f);
+    const float3 F     = F0 + (f3(1, 1, 1) - F0) * p5;
+    if (spec)
+    {
+        const float a2  = (roughness * roughness) * (roughness * roughness), dd = (NdotH * NdotH) * (a2 - 1.0f) + 1.0f;
+        const float pdf = p_spec * ((a2 / (3.14159265359f * dd * dd)) * NdotH / (4.0f * VdotH)); // D_true(NH) NH / (4 VH), unclamped GGX
+        if (!(pdf > 0.0f)) return false;
+        const float sv = D_ggx(NdotH, roughness * roughness) * (G1_schlick_ggx(roughness, NdotL) * G1_schlick_ggx(roughness, NdotV)) / fmaxf(0.0001f, 4.0f * NdotL * NdotV);
+        weight = F * (sv * NdotL / pdf);
+    }
+    else
+    {
+        const float pdf = (1.0f - p_spec) * (NdotL / 3.14159265359f);
+        weight = ((f3(1, 1, 1) - F) * (cd * (1.0f / 3.14159265359f))) * (NdotL / pdf);
+    }
+    return true;
+}
+
 // warp = 8x4 pixel block (coherent primary rays), 2-warp CTAs like K12
-template <bool TEX>
+// INDIRECT = false: the reference as written (one vertex).  true: trace_indirect = 1, a per-lane bounce loop over up to max_ray_bounces
+// vertices (the wavefront split lost for K12 on this card, DESIGN.md §8); out_hash gets the path hash
+template <bool TEX, bool INDIRECT>
 __global__ void __launch_bounds__(64) k_path_trace(BvhDev bvh, ShadeDev sd, PathTraceParams P, const uint2* __restrict__ prev, uint2* __restrict__ out, uint32_t* __restrict__ out_prim,
-                                                   tex::TexDev T)
+                                                   tex::TexDev T, uint32_t* __restrict__ out_hash)
 {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int x = blockIdx.x * 16 + warp * 8 + (lane & 7), y = blockIdx.y * 4 + (lane >> 3);
@@ -423,47 +501,54 @@ __global__ void __launch_bounds__(64) k_path_trace(BvhDev bvh, ShadeDev sd, Path
     float    t, hu, hv;
     uint32_t prim = 0xFFFFFFFFu;
     count_rays(P.ray_ctr, 0, 1u);
-    if (trace_closest(bvh, r, t, prim, hu, hv))
-    { // rchit:112-141
-        using namespace gi;
-        const Surface s  = TEX ? fetch_surface_tex(sd, T, prim, hu, hv) : fetch_surface(sd, prim, hu, hv);
-        const float   roughness = s.roughness * P.roughness_multiplier;
-        const V3      Wo = det::scale(r.d, -1.0f);
-        const float3  F0 = f3(0.04f, 0.04f, 0.04f) * (1.0f - s.metallic) + s.albedo * s.metallic;
-        const float3  cd = (s.albedo * (f3(1, 1, 1) - F0)) * (1.0f - s.metallic) + f3(0, 0, 0) * s.metallic;
-        const float   r1x = next_float(rng), r1y = next_float(rng); // next_vec2: the light's disk sample
-        const float   r2x = next_float(rng), r2y = next_float(rng); // next_vec2: the sky sample
-        // direct_lighting, lighting.glsl:117-196 with SOFT_SHADOWS, RAY_THROUGHPUT (T = 1 at depth 0), SAMPLE_SKY_LIGHT
-        float3 Lo = f3(0, 0, 0);
-        Ray    sr;
-        sr.o    = det::add(s.P, det::scale(s.N, 0.1f));
-        sr.tmin = 0.01f;
+    if (!INDIRECT)
+    {
+        if (trace_closest(bvh, r, t, prim, hu, hv))
+        { // rchit:112-141
+            using namespace gi;
+            const Surface s  = TEX ? fetch_surface_tex(sd, T, prim, hu, hv) : fetch_surface(sd, prim, hu, hv);
+            const float   roughness = s.roughness * P.roughness_multiplier;
+            const V3      Wo = det::scale(r.d, -1.0f);
+            const float3  F0 = f3(0.04f, 0.04f, 0.04f) * (1.0f - s.metallic) + s.albedo * s.metallic;
+            const float3  cd = (s.albedo * (f3(1, 1, 1) - F0)) * (1.0f - s.metallic) + f3(0, 0, 0) * s.metallic;
+            // RAY_THROUGHPUT: T = 1 at depth 0
+            L = path_direct_lighting(bvh, P, s, roughness, Wo, F0, cd, sky, rng); // + indirect_lighting(...) = vec3(0): the bounce is commented out in the reference (rchit:92-106)
+        }
+    }
+    else
+    {
+        uint32_t hash = 2166136261u, end = PT_END_MISS;
+        if (trace_closest(bvh, r, t, prim, hu, hv))
         {
-            const hr_light& light = P.light;
-            const float3    Li = make_float3(light.data2[0] * light.data0[3], light.data2[1] * light.data0[3], light.data2[2] * light.data0[3]);
-            V3    Wi;
-            float t_max, att;
-            det::fetch_light_properties_shadow(light, s.P, s.N, r1x, r1y, Wi, t_max, att);
-            const V3 Wh = det::normalize(det::add(Wo, Wi));
-            if (att > 0.0f)
+            using namespace gi;
+            float3   Tp = f3(1, 1, 1);
+            uint32_t hp = prim;
+            L = f3(0, 0, 0);
+#pragma unroll 1
+            for (uint32_t k = 0;; k++)
             {
-                sr.d    = Wi;
-                sr.tmax = t_max;
+                hash = fnv1a(hash, hp);
+                const Surface s  = TEX ? fetch_surface_tex(sd, T, hp, hu, hv) : fetch_surface(sd, hp, hu, hv);
+                const float   roughness = s.roughness * P.roughness_multiplier;
+                const V3      Wo = det::scale(r.d, -1.0f);
+                const float3  F0 = f3(0.04f, 0.04f, 0.04f) * (1.0f - s.metallic) + s.albedo * s.metallic;
+                const float3  cd = (s.albedo * (f3(1, 1, 1) - F0)) * (1.0f - s.metallic) + f3(0, 0, 0) * s.metallic;
+                L = L + Tp * path_direct_lighting(bvh, P, s, roughness, Wo, F0, cd, sky, rng);
+                if (k + 1 == P.max_ray_bounces) { end = PT_END_MAX_BOUNCES; break; }
+                const float u = next_float(rng), e1 = next_float(rng), e2 = next_float(rng);
+                float3      weight;
+                V3          Wi;
+                if (!sample_bounce(s.N, Wo, F0, cd, roughness, s.metallic, u, e1, e2, Wi, weight)) { end = PT_END_HORIZON; break; }
+                Tp     = Tp * weight;
+                r.o    = det::add(s.P, det::scale(s.N, 0.1f)); // the shadow-ray origin, lighting.glsl:143
+                r.d    = Wi;
+                r.tmin = 0.001f;
+                r.tmax = 10000.0f;
                 count_rays(P.ray_ctr, 1, 1u);
-                att *= trace_any(bvh, sr) ? 0.0f : 1.0f;
+                if (!trace_closest(bvh, r, t, hp, hu, hv)) { end = PT_END_MISS; break; } // rmiss adds the environment at depth 0 only
             }
-            Lo = Lo + (evaluate_uber_brdf(cd, roughness, s.N, F0, Wo, Wh, Wi) * att) * Li;
         }
-        {
-            const V3 Wi = det::sample_cosine_lobe(s.N, r2x, r2y);
-            const V3 Wh = det::normalize(det::add(Wo, Wi));
-            sr.d    = Wi;
-            sr.tmax = 10000.0f;
-            count_rays(P.ray_ctr, 1, 1u);
-            const float vis = trace_any(bvh, sr) ? 0.0f : 1.0f;
-            Lo = Lo + evaluate_uber_brdf(cd, roughness, s.N, F0, Wo, Wh, Wi) * (sky * vis);
-        }
-        L = Lo; // + indirect_lighting(...) = vec3(0): the bounce is commented out in the reference (rchit:92-106)
+        out_hash[idx] = fnv1a(hash, end);
     }
     // rgen:94-111: clamp to RADIANCE_CLAMP_COLOR = 1, then the running average the reference writes (weight 1 / num_frames, not 1 / (n + 1))
     const float3 c = make_float3(fminf(L.x, 1.0f), fminf(L.y, 1.0f), fminf(L.z, 1.0f));
@@ -536,7 +621,7 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
 }
 
 void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       const void* prev, void* out, uint32_t* out_prim, unsigned long long* ray_ctr, cudaStream_t st)
+                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, cudaStream_t st)
 {
     PathTraceParams P;
     memcpy(P.view_inverse, f->ubo.view_inverse, 64);
@@ -547,6 +632,14 @@ void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint
     P.W = W; P.H = H;
     P.ray_ctr = ray_ctr;
     dim3 grid((W + 15) / 16, (H + 3) / 4);
-    if (sc->tex.n_textures > 0) k_path_trace<true><<<grid, 64, 0, st>>>(hr_bvh_view(sc), shade_view(sc), P, (const uint2*)prev, (uint2*)out, out_prim, sc->tex);
-    else k_path_trace<false><<<grid, 64, 0, st>>>(hr_bvh_view(sc), shade_view(sc), P, (const uint2*)prev, (uint2*)out, out_prim, sc->tex);
+#define HR_PT_ARGS hr_bvh_view(sc), shade_view(sc), P, (const uint2*)prev, (uint2*)out, out_prim, sc->tex
+    const bool textured = sc->tex.n_textures > 0; // material textures change the lobe inputs: both indirect forms have a TEX instantiation
+    if (trace_indirect)
+    {
+        if (textured) k_path_trace<true, true><<<grid, 64, 0, st>>>(HR_PT_ARGS, out_hash);
+        else k_path_trace<false, true><<<grid, 64, 0, st>>>(HR_PT_ARGS, out_hash);
+    }
+    else if (textured) k_path_trace<true, false><<<grid, 64, 0, st>>>(HR_PT_ARGS, nullptr);
+    else k_path_trace<false, false><<<grid, 64, 0, st>>>(HR_PT_ARGS, nullptr);
+#undef HR_PT_ARGS
 }

@@ -332,6 +332,8 @@ public:
     void     restart_accumulation() { hr_pass_reset_history(m_pass); } // ground_truth_path_tracer.h:17
     hr_image output_ds() const { hr_image img {}; check(m_common->ctx, hr_pass_output(m_pass, HR_PATH_TRACER_OUT_FINAL, &img), "hr_pass_output"); return img; }
     hr_pass* handle() { return m_pass; }
+    // params.trace_indirect = 1 traces the indirect bounces up to params.max_ray_bounces path vertices; 0 (the default) renders the
+    // reference as written, direct light plus one sky sample (hr_path_tracer_params)
     hr_path_tracer_params params;
 private:
     CommonResources* m_common;

@@ -706,11 +706,13 @@ class TonemapPass(Pass):
 
 
 class hr_path_tracer_params(C.Structure):
-    _fields_ = [("max_ray_bounces", C.c_int32), ("roughness_multiplier", C.c_float), ("sky_color", C.c_float * 3)]
+    _fields_ = [("max_ray_bounces", C.c_int32), ("roughness_multiplier", C.c_float), ("sky_color", C.c_float * 3), ("trace_indirect", C.c_int32)]
 
 
 class PathTracerPass(Pass):
-    """ground-truth progressive path tracer (hr_path_tracer_*); reset_history() = restart_accumulation()"""
+    """ground-truth progressive path tracer (hr_path_tracer_*); reset_history() = restart_accumulation().  params.trace_indirect = 1 traces
+    the indirect bounces up to params.max_ray_bounces path vertices (0, the default, is the reference as written); download(2) is then the
+    path hash (HR_PATH_TRACER_OUT_PATH_HASH)"""
 
     def __init__(self, ctx: Context, W, H):
         self.ctx, self.kind, self.lib = ctx, "path_tracer", ctx.lib

@@ -470,17 +470,28 @@ HR_API int hr_tonemap_render(hr_pass* pass, const hr_tonemap_params* params, hr_
  * Ground-truth progressive path tracer  (SURVEY.md §8 f4: src/ground_truth_path_tracer.{h,cpp}; shaders/ground_truth/ *)
  * One jittered primary ray per pixel per render; first hit shaded with the soft-shadowed punctual light and one cosine-lobe sky
  * sample (each with its shadow ray); running average over renders.  As written in the reference the indirect bounce is disabled
- * (its traceRayEXT is commented out, ground_truth_path_trace.rchit:92-104), so max_ray_bounces changes nothing.  Needs only the
+ * (its traceRayEXT is commented out, ground_truth_path_trace.rchit:92-104), so max_ray_bounces changes nothing unless trace_indirect
+ * is 1.  Needs only the
  * scene and frame->ubo.{view_inverse, proj_inverse, light}: no G-buffer.  Replicated (not sharded) when world > 1.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct hr_path_tracer_params {
     int32_t max_ray_bounces;      /* 2 (ground_truth_path_tracer.h:28; the ctor overwrites it with the device's recursion limit) */
     float   roughness_multiplier; /* 1.0 (CommonResources::roughness_multiplier, common.h:193) */
     float   sky_color[3];         /* constant-colour environment replacing the sky cubemap */
+    int32_t trace_indirect;       /* 0 = the reference as written (default): one path vertex, direct light + one sky sample.  1 = what the
+                                   * code evidently intends (max_ray_bounces, RAY_THROUGHPUT, the environment added at depth 0 only): each
+                                   * vertex adds direct_lighting weighted by the path throughput, then samples the GGX or the diffuse lobe
+                                   * and traces the bounce, up to max_ray_bounces vertices (1 = direct light only, bit for bit the image of
+                                   * 0; 2 = one indirect bounce).  Requires 1 <= max_ray_bounces <= 31 (the recursion limit the reference
+                                   * reads on NVIDIA devices).  No Russian roulette; estimator in DESIGN.md §7 */
 } hr_path_tracer_params;
 enum {
     HR_PATH_TRACER_OUT_COLOR     = 0,  /* RGBA16F running average (rgb clamped to 1 per sample, a = 1) */
     HR_PATH_TRACER_OUT_PRIMITIVE = 1,  /* R32_UINT primitive hit by the last render's primary ray, 0xFFFFFFFF = sky (tests) */
+    HR_PATH_TRACER_OUT_PATH_HASH = 2,  /* R32_UINT, trace_indirect = 1 renders only (tests): FNV-1a, h = (h ^ w) * 16777619 from 2166136261,
+                                        * over the primitive hit by every path segment in order (primary included), then one end code:
+                                        * 0xFFFFFFFF the last ray missed, 0xFFFFFFFE the sampled direction was below the horizon,
+                                        * 0xFFFFFFFD the path reached max_ray_bounces */
     HR_PATH_TRACER_OUT_FINAL     = 100
 };
 HR_API void hr_path_tracer_default_params(hr_path_tracer_params* p);
