@@ -12,12 +12,7 @@ static std::string g_last_error;
 static std::mutex  g_err_mutex;
 extern int         g_hr_atrous_impl;
 extern int         g_hr_bvh_quality;
-extern int         g_hr_force_shared_rt;
-extern int         g_hr_atrous_rows;
 extern int         g_hr_refl_atrous_impl;
-extern int         g_hr_refl_atrous_minb;
-extern int         g_hr_gather_impl;
-extern int         g_hr_force_peer_temporal;
 
 void hr_set_error(hr_ctx* ctx, const char* fmt, ...)
 {
@@ -164,14 +159,9 @@ const char* hr_last_error(hr_ctx* ctx)
 
 int hr_debug_set(int key, int value)
 {
-    if (key == 1) { g_hr_atrous_impl = value; return HR_OK; }
-    if (key == 3) { g_hr_bvh_quality = value; return HR_OK; }
-    if (key == 4) { g_hr_force_shared_rt = value; return HR_OK; }
-    if (key == 5) { g_hr_atrous_rows = value; return HR_OK; }
-    if (key == 6) { g_hr_refl_atrous_impl = value; return HR_OK; }
-    if (key == 8) { g_hr_refl_atrous_minb = value; return HR_OK; }
-    if (key == 11) { g_hr_gather_impl = value; return HR_OK; }
-    if (key == 12) { g_hr_force_peer_temporal = value; return HR_OK; }
+    if (key == 1 && (value == 0 || value == 1 || value == 3)) { g_hr_atrous_impl = value; return HR_OK; }
+    if (key == 3 && (value == 0 || value == 1)) { g_hr_bvh_quality = value; return HR_OK; }
+    if (key == 6 && (value == 0 || value == 2 || value == 3)) { g_hr_refl_atrous_impl = value; return HR_OK; }
     return HR_ERR_INVALID_ARG;
 }
 

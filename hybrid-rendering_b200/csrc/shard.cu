@@ -13,9 +13,9 @@
 //     after its last history write of frame N a rank stores N into every peer's tick array (st.release.sys); before
 //     the reprojection of frame N+1 a one-warp kernel spins (ld.acquire.sys, 10 s time-out) until every peer's tick
 //     is >= N.  History images are double buffered by frame parity, so that wait also covers the write-after-read hazard.
-//   * the pass's FINAL OUTPUT (optional, hr_shard_set_gather; on by default): one NCCL group of per-band broadcasts (an
+//   * the pass's FINAL OUTPUT (optional, hr_shard_set_gather; on by default): one NCCL group of point-to-point transfers (an
 //     all-gather with unequal counts: 2160 rows = 270 tiles do not divide evenly by 8) on a side stream, so every rank
-//     ends up with the complete denoised frame.  The reflections / DDGI passes still exchange their history this way.
+//     ends up with the complete denoised frame.  DDGI exchanges its updated probe rows with per-band broadcasts.
 // The 1/2/4/8-GPU results are bit-identical to the single-GPU result (tests/test_gpu_multi.py).
 //
 // NCCL is dlopen'ed on first use so the single-GPU library has no NCCL dependency; inside a PyTorch process the
@@ -36,8 +36,8 @@ struct NcclApi {
     ncclResult_t (*GroupEnd)()                                                                                 = nullptr;
     ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)       = nullptr;
     ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t)            = nullptr;
-    ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                   = nullptr; // optional
-    ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                         = nullptr; // optional
+    ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                   = nullptr; // NCCL 2.7+
+    ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                         = nullptr; // NCCL 2.7+
     const char* (*GetErrorString)(ncclResult_t)                                                                = nullptr;
     bool ok = false;
 };
@@ -65,7 +65,8 @@ NcclApi& nccl()
     LOAD(Recv, "ncclRecv");
     LOAD(GetErrorString, "ncclGetErrorString");
 #undef LOAD
-    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.GroupStart && api.GroupEnd && api.Broadcast && api.AllGather && api.GetErrorString;
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.GroupStart && api.GroupEnd && api.Broadcast && api.AllGather && api.Send && api.Recv &&
+             api.GetErrorString;
     return api;
 }
 
@@ -79,10 +80,6 @@ NcclApi& nccl()
             return HR_ERR_NCCL;                                                                                 \
         }                                                                                                       \
     } while (0)
-
-// How the final-output gather moves the bands: 0 = one ncclBroadcast per band, 1 = point-to-point (every rank sends its band to
-// each peer and receives theirs: 7 independent NVSwitch transfers per rank instead of 8 serial broadcast rings).  hr_debug_set key 11.
-int g_hr_gather_impl = 1;
 
 void hr_band(const hr_ctx* ctx, int H, int* b0, int* b1)
 {
@@ -122,14 +119,12 @@ int hr_shard_exchange(hr_pass* p, const ExchangeItem* items, int n, cudaStream_t
             if (re <= rb) continue;
             char*        p     = static_cast<char*>(items[i].base) + (size_t)rb * items[i].row_bytes;
             const size_t bytes = (size_t)(re - rb) * items[i].row_bytes;
-            if (g_hr_gather_impl == 1 && N.Send && N.Recv)
-            {
-                if (r != ctx->rank) HR_NCCL(ctx, N.Recv(p, bytes, ncclUint8, r, (ncclComm_t)ctx->nccl_comm, st));
-                else
-                    for (int q = 0; q < ctx->world; q++)
-                        if (q != ctx->rank) HR_NCCL(ctx, N.Send(p, bytes, ncclUint8, q, (ncclComm_t)ctx->nccl_comm, st));
-            }
-            else HR_NCCL(ctx, N.Broadcast(p, p, bytes, ncclUint8, r, (ncclComm_t)ctx->nccl_comm, st));
+            // point to point: every rank sends its band to each peer and receives theirs (7 independent NVSwitch transfers per
+            // rank instead of 8 serial broadcast rings)
+            if (r != ctx->rank) HR_NCCL(ctx, N.Recv(p, bytes, ncclUint8, r, (ncclComm_t)ctx->nccl_comm, st));
+            else
+                for (int q = 0; q < ctx->world; q++)
+                    if (q != ctx->rank) HR_NCCL(ctx, N.Send(p, bytes, ncclUint8, q, (ncclComm_t)ctx->nccl_comm, st));
         }
     HR_NCCL(ctx, N.GroupEnd());
     HR_CUDA(ctx, cudaEventRecord(p->ev_done, st));
@@ -520,18 +515,10 @@ static int rt_init_bounds(hr_pass* p)
     return HR_OK;
 }
 
-int g_hr_force_shared_rt = 0; // hr_debug_set(4, 1): run the cooperative ray-trace kernel on a single GPU (overhead A/B)
-
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out)
 {
     hr_ctx* ctx = p->ctx;
-    const bool forced = g_hr_force_shared_rt && ctx->world == 1 && p->n_hist >= 7;
-    if (forced && !p->hist_peer[0][6])
-    {
-        for (int k = 0; k < p->n_hist; k++) p->hist_peer[0][k] = p->hist_local[k];
-        if (rt_init_bounds(p) != HR_OK) return false;
-    }
-    if (!forced && (!p->peers_linked || ctx->world <= 1 || p->n_hist < 7)) return false;
+    if (!p->peers_linked || ctx->world <= 1 || p->n_hist < 7) return false;
     RtShare sh {};
     sh.mask_local = static_cast<uint32_t*>(p->hist_local[4 + parity]);
     sh.bounds     = p->rt_bounds;
@@ -555,7 +542,7 @@ int hr_rt_share_finish(hr_pass* p, int parity, int tick, cudaStream_t st)
         m.p[r] = static_cast<uint32_t*>(p->hist_peer[r][4 + parity]);
         t.p[r] = p->peer_ticks[r];
     }
-    k_rt_push<<<ctx->world > 1 ? 32 : 1, 256, 0, st>>>(m, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, MW, tick);
+    k_rt_push<<<32, 256, 0, st>>>(m, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, MW, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -564,16 +551,13 @@ int hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cud
 {
     hr_ctx*   ctx = p->ctx;
     const int MH  = (p->H + 3) / 4;
-    int*      d_err = nullptr;
-    if (ctx->world > 1)
+    if (p->sync_error && *p->sync_error)
     {
-        if (p->sync_error && *p->sync_error)
-        {
-            hr_set_error(ctx, "peer sync: timed out waiting for rank %d's frame tick (peer stopped, or ranks rendered different frame counts)", *p->sync_error - 1);
-            return HR_ERR_NCCL;
-        }
-        HR_CUDA(ctx, cudaHostGetDevicePointer((void**)&d_err, p->sync_error, 0));
+        hr_set_error(ctx, "peer sync: timed out waiting for rank %d's frame tick (peer stopped, or ranks rendered different frame counts)", *p->sync_error - 1);
+        return HR_ERR_NCCL;
     }
+    int* d_err = nullptr;
+    HR_CUDA(ctx, cudaHostGetDevicePointer((void**)&d_err, p->sync_error, 0));
     k_rt_wait_partition<<<1, 32, 0, st>>>(p->sync_ticks, rt_tick, hist_tick, d_err, p->rt_cost_all + (size_t)parity * MH, MH, ctx->world, ctx->rank,
                                          hr_rt_share_cap(MH, ctx->world), p->rt_bounds);
     ctx->launches++;

@@ -25,7 +25,7 @@ struct AtrousParams {
     int   row0, row1;
 };
 
-// ---- naive reference kernel (global memory only); kept for A/B validation of the tiled kernel -------------------
+// ---- naive kernel (global memory only): the fallback for radius != 1 and steps >= 16, and hr_debug_set(1, 0) ------
 __global__ void __launch_bounds__(256) k_atrous_naive(GBufLevelDev g, const uint32_t* __restrict__ in, const uint8_t* __restrict__ tile_flags,
                                                        AtrousParams P, uint32_t* __restrict__ out)
 {

@@ -33,6 +33,9 @@ __device__ __forceinline__ float2 ld_pair(const float* __restrict__ plane, int i
 
 struct PairCell { float2 nx, ny, nz, zs, vis, var; };
 
+// the six staged planes of a tile region
+struct Planes { const float *nx, *ny, *nz, *zs, *vi, *va; };
+
 // Stage the texel pair (px, px+1) of row py (px even) into the six planes at region index ri (even): decoded normal,
 // scaled linear depth, visibility, variance; zeros outside the image (zero normal = weight 0, the reference's `inside`).
 __device__ __forceinline__ void stage_pair(const GBufLevelDev& g, const uint32_t* __restrict__ in, float c_sigma, int px, int py, int W, int H, int ri, float* s_nx,
@@ -54,6 +57,80 @@ __device__ __forceinline__ void stage_pair(const GBufLevelDev& g, const uint32_t
     }
     *reinterpret_cast<float2*>(s_nx + ri) = nx; *reinterpret_cast<float2*>(s_ny + ri) = ny; *reinterpret_cast<float2*>(s_nz + ri) = nz;
     *reinterpret_cast<float2*>(s_zs + ri) = zs; *reinterpret_cast<float2*>(s_vi + ri) = vi; *reinterpret_cast<float2*>(s_va + ri) = va;
+}
+
+// Filter the pixel pair whose centre cell is at region index ci and store it at out[idx] (and out[idx + 1] when has1); row /
+// column tap strides in cells are (rs, cs).  up / dn: the cells directly above / below the centre at UNIT pixel spacing in a
+// variance plane (the dense tile keeps them in its main variance plane, the row-interleaved tile in side buffers).
+template <bool ALIGNED_X>
+__device__ __forceinline__ void filter_store_pair(const Planes& s, int ci, int rs, int cs, const float* up, const float* dn, const V3Params& P,
+                                                  uint32_t* __restrict__ out, size_t idx, bool has1)
+{
+    const float2 neg1 = make_float2(-1.0f, -1.0f), nl2e = make_float2(-1.44269504f, -1.44269504f);
+    const float  LK1 = -0.5849625007f, LK2 = -1.1699250014f; // log2(2/3), log2(4/9): kernel weights folded into the exponent
+    PairCell     c;
+    c.nx = ld_pair(s.nx, ci, true); c.ny = ld_pair(s.ny, ci, true); c.nz = ld_pair(s.nz, ci, true);
+    c.zs = ld_pair(s.zs, ci, true); c.vis = ld_pair(s.vi, ci, true); c.var = ld_pair(s.va, ci, true);
+    // compute_variance_center for both pixels: columns ci-1 .. ci+2, rows -1..+1; weights {1/4,1/8,1/16}
+    float2 vbar;
+    {
+        const float  a0 = up[-1], d0 = up[2];
+        const float2 m0 = *reinterpret_cast<const float2*>(up);
+        const float  a1 = s.va[ci - 1], d1 = s.va[ci + 2];
+        const float  a2 = dn[-1], d2 = dn[2];
+        const float2 m2 = *reinterpret_cast<const float2*>(dn);
+        vbar.x = 0.25f * c.var.x + 0.125f * (a1 + c.var.y + m0.x + m2.x) + 0.0625f * (a0 + m0.y + a2 + m2.y);
+        vbar.y = 0.25f * c.var.y + 0.125f * (c.var.x + d1 + m0.y + m2.y) + 0.0625f * (m0.x + d0 + m2.x + d2);
+    }
+    const float2 cphi = make_float2(P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.x, 1e-30f)), P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.y, 1e-30f)));
+    float2 sumw = make_float2(1.0f, 1.0f), s0 = c.vis, s1 = c.var;
+#pragma unroll
+    for (int yy = -1; yy <= 1; yy++)
+#pragma unroll
+        for (int xx = -1; xx <= 1; xx++)
+        {
+            if (xx == 0 && yy == 0) continue;
+            const float lk      = (xx != 0 && yy != 0) ? LK2 : LK1;
+            const int   si      = ci + yy * rs + xx * cs;
+            const bool  aligned = ALIGNED_X || xx == 0;
+            PairCell    t;
+            t.nx = ld_pair(s.nx, si, aligned); t.ny = ld_pair(s.ny, si, aligned); t.nz = ld_pair(s.nz, si, aligned);
+            t.zs = ld_pair(s.zs, si, aligned); t.vis = ld_pair(s.vi, si, aligned); t.var = ld_pair(s.va, si, aligned);
+            const float2 dz = ffma2(t.zs, neg1, c.zs);
+            float2       wZ;
+            wZ.x = fast_exp2(-fabsf(dz.x));
+            wZ.y = fast_exp2(-fabsf(dz.y));
+            const float2 dl = ffma2(t.vis, neg1, c.vis);
+            float2       ea;
+            ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
+            ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
+            ea   = ffma2(wZ, nl2e, ea);
+            float2 e;
+            e.x = fast_exp2(ea.x);
+            e.y = fast_exp2(ea.y);
+            float2 nd = fmul2(c.nz, t.nz);
+            nd        = ffma2(c.ny, t.ny, nd);
+            nd        = ffma2(c.nx, t.nx, nd);
+            nd.x      = fmaxf(nd.x, 0.0f);
+            nd.y      = fmaxf(nd.y, 0.0f);
+            float2 p = fmul2(nd, nd);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            p        = fmul2(p, p);
+            const float2 wk = fmul2(e, p);
+            sumw = fadd2(sumw, wk);
+            s0   = ffma2(wk, t.vis, s0);
+            s1   = ffma2(fmul2(wk, wk), t.var, s1);
+        }
+    const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
+    float2       o0 = fmul2(s0, inv), o1 = fmul2(fmul2(s1, inv), inv);
+    if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
+    // sky pixels (linear z < 0) pass the input through
+    const uint32_t r0 = c.zs.x < 0.0f ? f2_to_h2(c.vis.x, c.var.x) : f2_to_h2(o0.x, o1.x);
+    const uint32_t r1 = c.zs.y < 0.0f ? f2_to_h2(c.vis.y, c.var.y) : f2_to_h2(o0.y, o1.y);
+    if (has1) *reinterpret_cast<uint2*>(out + idx) = make_uint2(r0, r1); // idx even (W even is required by the launcher)
+    else out[idx] = r0;
 }
 
 template <int STEP>
@@ -99,10 +176,9 @@ __global__ void __launch_bounds__(256) k_atrous_v3(GBufLevelDev g, const uint32_
     }
     __syncthreads();
 
-    const int lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5; // 32 pixel pairs x 8 rows, 2 rows per thread
-    const int x = x0 + 2 * lx2;
-    const float2 neg1 = make_float2(-1.0f, -1.0f), nl2e = make_float2(-1.44269504f, -1.44269504f);
-    const float  LK1 = -0.5849625007f, LK2 = -1.1699250014f; // log2(2/3), log2(4/9): kernel weights folded into the exponent
+    const Planes pl { s_nx, s_ny, s_nz, s_zs, s_vi, s_va };
+    const int    lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5; // 32 pixel pairs x 8 rows, 2 rows per thread
+    const int    x = x0 + 2 * lx2;
 #pragma unroll
     for (int k = 0; k < TH3 / 8; k++)
     {
@@ -117,69 +193,7 @@ __global__ void __launch_bounds__(256) k_atrous_v3(GBufLevelDev g, const uint32_
             continue;
         }
         const int ci = (ly + STEP) * RW + 2 * lx2 + PADL;
-        PairCell  c;
-        c.nx = ld_pair(s_nx, ci, true); c.ny = ld_pair(s_ny, ci, true); c.nz = ld_pair(s_nz, ci, true);
-        c.zs = ld_pair(s_zs, ci, true); c.vis = ld_pair(s_vi, ci, true); c.var = ld_pair(s_va, ci, true);
-        // compute_variance_center for both pixels: columns ci-1 .. ci+2, rows -1..+1; weights {1/4,1/8,1/16}
-        float2 vbar;
-        {
-            const float a0 = s_va[ci - RW - 1], d0 = s_va[ci - RW + 2];
-            const float2 m0 = ld_pair(s_va, ci - RW, true);
-            const float a1 = s_va[ci - 1], d1 = s_va[ci + 2];
-            const float a2 = s_va[ci + RW - 1], d2 = s_va[ci + RW + 2];
-            const float2 m2 = ld_pair(s_va, ci + RW, true);
-            vbar.x = 0.25f * c.var.x + 0.125f * (a1 + c.var.y + m0.x + m2.x) + 0.0625f * (a0 + m0.y + a2 + m2.y);
-            vbar.y = 0.25f * c.var.y + 0.125f * (c.var.x + d1 + m0.y + m2.y) + 0.0625f * (m0.x + d0 + m2.x + d2);
-        }
-        const float2 cphi = make_float2(P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.x, 1e-30f)), P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.y, 1e-30f)));
-        float2 sumw = make_float2(1.0f, 1.0f), s0 = c.vis, s1 = c.var;
-#pragma unroll
-        for (int yy = -1; yy <= 1; yy++)
-#pragma unroll
-            for (int xx = -1; xx <= 1; xx++)
-            {
-                if (xx == 0 && yy == 0) continue;
-                const float lk      = (xx != 0 && yy != 0) ? LK2 : LK1;
-                const int   si      = ci + yy * STEP * RW + xx * STEP;
-                const bool  aligned = ((xx * STEP) & 1) == 0;
-                PairCell    s;
-                s.nx = ld_pair(s_nx, si, aligned); s.ny = ld_pair(s_ny, si, aligned); s.nz = ld_pair(s_nz, si, aligned);
-                s.zs = ld_pair(s_zs, si, aligned); s.vis = ld_pair(s_vi, si, aligned); s.var = ld_pair(s_va, si, aligned);
-                const float2 dz = ffma2(s.zs, neg1, c.zs);
-                float2       wZ;
-                wZ.x = fast_exp2(-fabsf(dz.x));
-                wZ.y = fast_exp2(-fabsf(dz.y));
-                const float2 dl = ffma2(s.vis, neg1, c.vis);
-                float2       ea;
-                ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
-                ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-                ea   = ffma2(wZ, nl2e, ea);
-                float2 e;
-                e.x = fast_exp2(ea.x);
-                e.y = fast_exp2(ea.y);
-                float2 nd = fmul2(c.nz, s.nz);
-                nd        = ffma2(c.ny, s.ny, nd);
-                nd        = ffma2(c.nx, s.nx, nd);
-                nd.x      = fmaxf(nd.x, 0.0f);
-                nd.y      = fmaxf(nd.y, 0.0f);
-                float2 p = fmul2(nd, nd);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                const float2 wk = fmul2(e, p);
-                sumw = fadd2(sumw, wk);
-                s0   = ffma2(wk, s.vis, s0);
-                s1   = ffma2(fmul2(wk, wk), s.var, s1);
-            }
-        const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-        float2       o0 = fmul2(s0, inv), o1 = fmul2(fmul2(s1, inv), inv);
-        if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
-        // sky pixels (linear z < 0) pass the input through
-        const uint32_t r0 = c.zs.x < 0.0f ? f2_to_h2(c.vis.x, c.var.x) : f2_to_h2(o0.x, o1.x);
-        const uint32_t r1 = c.zs.y < 0.0f ? f2_to_h2(c.vis.y, c.var.y) : f2_to_h2(o0.y, o1.y);
-        if (has1) *reinterpret_cast<uint2*>(out + idx) = make_uint2(r0, r1); // idx even (W even is required by the launcher)
-        else out[idx] = r0;
+        filter_store_pair<(STEP & 1) == 0>(pl, ci, STEP * RW, STEP, s_va + ci - RW, s_va + ci + RW, P, out, idx, has1);
     }
 }
 
@@ -249,10 +263,9 @@ __global__ void __launch_bounds__(256) k_atrous_v3s(GBufLevelDev g, const uint32
     }
     __syncthreads();
 
-    const int lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5; // 32 pixel pairs x 8 rows, 2 rows per thread
-    const int x = x0 + 2 * lx2;
-    const float2 neg1 = make_float2(-1.0f, -1.0f), nl2e = make_float2(-1.44269504f, -1.44269504f);
-    const float  LK1 = -0.5849625007f, LK2 = -1.1699250014f; // log2(2/3), log2(4/9): kernel weights folded into the exponent
+    const Planes pl { s_nx, s_ny, s_nz, s_zs, s_vi, s_va };
+    const int    lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5; // 32 pixel pairs x 8 rows, 2 rows per thread
+    const int    x = x0 + 2 * lx2;
 #pragma unroll
     for (int k = 0; k < TH3 / 8; k++)
     {
@@ -267,68 +280,7 @@ __global__ void __launch_bounds__(256) k_atrous_v3s(GBufLevelDev g, const uint32
             continue;
         }
         const int ci = (ly + 1) * RW + 2 * lx2 + PADL;
-        PairCell  c;
-        c.nx = ld_pair(s_nx, ci, true); c.ny = ld_pair(s_ny, ci, true); c.nz = ld_pair(s_nz, ci, true);
-        c.zs = ld_pair(s_zs, ci, true); c.vis = ld_pair(s_vi, ci, true); c.var = ld_pair(s_va, ci, true);
-        float2 vbar;
-        {
-            const float* up = s_vadj + (0 * TH3 + ly) * RW + 2 * lx2 + PADL;
-            const float* dn = s_vadj + (1 * TH3 + ly) * RW + 2 * lx2 + PADL;
-            const float  a0 = up[-1], d0 = up[2];
-            const float2 m0 = *reinterpret_cast<const float2*>(up);
-            const float  a1 = s_va[ci - 1], d1 = s_va[ci + 2];
-            const float  a2 = dn[-1], d2 = dn[2];
-            const float2 m2 = *reinterpret_cast<const float2*>(dn);
-            vbar.x = 0.25f * c.var.x + 0.125f * (a1 + c.var.y + m0.x + m2.x) + 0.0625f * (a0 + m0.y + a2 + m2.y);
-            vbar.y = 0.25f * c.var.y + 0.125f * (c.var.x + d1 + m0.y + m2.y) + 0.0625f * (m0.x + d0 + m2.x + d2);
-        }
-        const float2 cphi = make_float2(P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.x, 1e-30f)), P.c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.y, 1e-30f)));
-        float2 sumw = make_float2(1.0f, 1.0f), s0 = c.vis, s1 = c.var;
-#pragma unroll
-        for (int yy = -1; yy <= 1; yy++)
-#pragma unroll
-            for (int xx = -1; xx <= 1; xx++)
-            {
-                if (xx == 0 && yy == 0) continue;
-                const float lk = (xx != 0 && yy != 0) ? LK2 : LK1;
-                const int   si = ci + yy * RW + xx * STEP;
-                PairCell    s;
-                s.nx = ld_pair(s_nx, si, true); s.ny = ld_pair(s_ny, si, true); s.nz = ld_pair(s_nz, si, true);
-                s.zs = ld_pair(s_zs, si, true); s.vis = ld_pair(s_vi, si, true); s.var = ld_pair(s_va, si, true);
-                const float2 dz = ffma2(s.zs, neg1, c.zs);
-                float2       wZ;
-                wZ.x = fast_exp2(-fabsf(dz.x));
-                wZ.y = fast_exp2(-fabsf(dz.y));
-                const float2 dl = ffma2(s.vis, neg1, c.vis);
-                float2       ea;
-                ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
-                ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-                ea   = ffma2(wZ, nl2e, ea);
-                float2 e;
-                e.x = fast_exp2(ea.x);
-                e.y = fast_exp2(ea.y);
-                float2 nd = fmul2(c.nz, s.nz);
-                nd        = ffma2(c.ny, s.ny, nd);
-                nd        = ffma2(c.nx, s.nx, nd);
-                nd.x      = fmaxf(nd.x, 0.0f);
-                nd.y      = fmaxf(nd.y, 0.0f);
-                float2 p = fmul2(nd, nd);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                p        = fmul2(p, p);
-                const float2 wk = fmul2(e, p);
-                sumw = fadd2(sumw, wk);
-                s0   = ffma2(wk, s.vis, s0);
-                s1   = ffma2(fmul2(wk, wk), s.var, s1);
-            }
-        const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-        float2       o0 = fmul2(s0, inv), o1 = fmul2(fmul2(s1, inv), inv);
-        if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
-        const uint32_t r0 = c.zs.x < 0.0f ? f2_to_h2(c.vis.x, c.var.x) : f2_to_h2(o0.x, o1.x);
-        const uint32_t r1 = c.zs.y < 0.0f ? f2_to_h2(c.vis.y, c.var.y) : f2_to_h2(o0.y, o1.y);
-        if (has1) *reinterpret_cast<uint2*>(out + idx) = make_uint2(r0, r1);
-        else out[idx] = r0;
+        filter_store_pair<true>(pl, ci, RW, STEP, s_vadj + (0 * TH3 + ly) * RW + 2 * lx2 + PADL, s_vadj + (1 * TH3 + ly) * RW + 2 * lx2 + PADL, P, out, idx, has1);
     }
 }
 
@@ -359,11 +311,6 @@ void launch_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, con
 
 } // namespace
 
-// 1 (default): step 8 uses the row-interleaved tiles (k_atrous_v3s); 2: steps 4 and 8; 0: dense tiles for every step
-// (hr_debug_set key 5).  Config 2 (1080p) on an H100 SXM 80 GB, 700 W power limit: step 8 interleaved 25.1 us vs dense 25.9; step 4
-// interleaved 24.3 us vs dense 22.1 (the two extra variance rows per filtered row cost more than the 8 halo rows they save).
-int g_hr_atrous_rows = 1;
-
 // returns false when this variant does not support the configuration (caller falls back to the scalar kernels)
 bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n, float sigma_z,
                               float power, uint32_t* out, int row0, int row1, cudaStream_t st)
@@ -374,8 +321,8 @@ bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const u
     {
         case 1: launch_v3<1>(g, in, tile_flags, P, out, st); break;
         case 2: launch_v3<2>(g, in, tile_flags, P, out, st); break;
-        case 4: if (g_hr_atrous_rows == 2) launch_v3s<4>(g, in, tile_flags, P, out, st); else launch_v3<4>(g, in, tile_flags, P, out, st); break;
-        default: if (g_hr_atrous_rows) launch_v3s<8>(g, in, tile_flags, P, out, st); else launch_v3<8>(g, in, tile_flags, P, out, st); break;
+        case 4: launch_v3<4>(g, in, tile_flags, P, out, st); break;
+        default: launch_v3s<8>(g, in, tile_flags, P, out, st); break; // row-interleaved tiles (DESIGN.md §8)
     }
     return true;
 }

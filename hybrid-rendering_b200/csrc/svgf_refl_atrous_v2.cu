@@ -14,8 +14,6 @@
 #include <cuda.h> // CUtensorMap (driver types only; cuTensorMapEncodeTiled is fetched with cudaGetDriverEntryPoint)
 #include <vector>
 
-int g_hr_refl_atrous_minb = 4; // hr_debug_set key 8: registers tuned for 4 (default: resident CTAs hide the staging latency), 3 or 2 CTAs per SM
-
 namespace {
 
 using namespace gf;
@@ -172,9 +170,9 @@ __device__ __forceinline__ void store_pair(uint2* __restrict__ out, size_t idx, 
     else out[idx] = r0;
 }
 
-// Dense tile: 64x16 pixels + STEP halo.  MINB = minimum resident CTAs per SM the register allocation is tuned for (A/B: hr_debug_set 8).
-template <int STEP, int MINB>
-__global__ void __launch_bounds__(256, MINB) k_refl_atrous_v2(GBufLevelDev g, const uint2* __restrict__ in, const uint8_t* __restrict__ tile_flags, R2Params P, uint2* __restrict__ out)
+// Dense tile: 64x16 pixels + STEP halo.  Registers are tuned for 4 resident CTAs per SM: they hide the staging latency.
+template <int STEP>
+__global__ void __launch_bounds__(256, 4) k_refl_atrous_v2(GBufLevelDev g, const uint2* __restrict__ in, const uint8_t* __restrict__ tile_flags, R2Params P, uint2* __restrict__ out)
 {
     extern __shared__ float smem_f[];
     constexpr int PADL = STEP + (STEP & 1);            // even left pad => even region column for even image column
@@ -331,24 +329,17 @@ __global__ void __launch_bounds__(256) k_refl_atrous_v2s(GBufLevelDev g, const u
     }
 }
 
-template <int STEP, int MINB>
-void launch_r2m(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, cudaStream_t st)
+template <int STEP>
+void launch_r2(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, cudaStream_t st)
 {
     constexpr int PADL = STEP + (STEP & 1);
     constexpr int RW   = (TWR + PADL + STEP + 1) & ~1;
     constexpr int RH   = THR + 2 * STEP;
     const size_t  smem = (size_t)RW * RH * NPL * sizeof(float);
     static bool   configured[64] = {};
-    if (hr_once_per_device(configured)) cudaFuncSetAttribute(k_refl_atrous_v2<STEP, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (hr_once_per_device(configured)) cudaFuncSetAttribute(k_refl_atrous_v2<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     dim3 grid((P.W + TWR - 1) / TWR, (P.row1 - P.row0 + THR - 1) / THR);
-    k_refl_atrous_v2<STEP, MINB><<<grid, 256, smem, st>>>(g, in, tf, P, out);
-}
-template <int STEP>
-void launch_r2(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, cudaStream_t st)
-{
-    if (g_hr_refl_atrous_minb == 2) launch_r2m<STEP, 2>(g, in, tf, P, out, st);
-    else if (g_hr_refl_atrous_minb == 3) launch_r2m<STEP, 3>(g, in, tf, P, out, st);
-    else launch_r2m<STEP, 4>(g, in, tf, P, out, st);
+    k_refl_atrous_v2<STEP><<<grid, 256, smem, st>>>(g, in, tf, P, out);
 }
 
 template <int STEP>
@@ -365,7 +356,7 @@ void launch_r2s(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const
 
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// TMA-staged, persistent form of the dense-tile kernel (steps 1, 2, 4).
+// TMA-staged, persistent form of the dense-tile kernel at step 1.
 //
 // k_refl_atrous_v2 issues far fewer instructions per iteration than the scalar kernel but stalls on long_scoreboard: every CTA
 // first waits for its own staging loads from DRAM (the images are larger than L2), and 2-4 resident CTAs per SM are not enough
@@ -395,8 +386,9 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, ui
                  : "memory");
 }
 
-template <int STEP>
+// the region of k_refl_atrous_v2<1>
 struct TmaGeom {
+    static constexpr int STEP = 1;
     static constexpr int PADL = STEP + (STEP & 1);
     static constexpr int RW   = (TWR + PADL + STEP + 1) & ~1;
     static constexpr int RH   = THR + 2 * STEP;
@@ -405,14 +397,13 @@ struct TmaGeom {
     static constexpr int SMEM = 3 * RAWB + NPL * PL * 4 + TWR * THR; // + one class byte per pixel of the tile
 };
 
-template <int STEP>
-__global__ void __launch_bounds__(256, (STEP <= 1 ? 3 : 2))
+__global__ void __launch_bounds__(256, 3)
 k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_constant__ CUtensorMap tm_gb3, const __grid_constant__ CUtensorMap tm_in, GBufLevelDev g,
                   const uint2* __restrict__ in, const uint8_t* __restrict__ tile_flags, R2Params P, uint2* __restrict__ out, int tiles_x, int n_tiles,
                   unsigned int* __restrict__ counter)
 {
-    using G = TmaGeom<STEP>;
-    constexpr int PADL = G::PADL, RW = G::RW, RH = G::RH, PL = G::PL;
+    using G = TmaGeom;
+    constexpr int STEP = G::STEP, PADL = G::PADL, RW = G::RW, RH = G::RH, PL = G::PL;
     extern __shared__ __align__(128) unsigned char smem_b[];
     unsigned char* raw0 = smem_b;
     float*         planes = reinterpret_cast<float*>(smem_b + 3 * G::RAWB);
@@ -588,13 +579,12 @@ bool tensor_map_2d(const void* ptr, int W, int H, int bw, int bh, CUtensorMap* o
     return true;
 }
 
-// counters: three words owned by the calling pass (one per step instantiation): passes of different contexts may run
-// concurrently on one device (emulated ranks on streams), so the tile counter cannot be a per-device static
-template <int STEP>
-bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, unsigned int* counters, cudaStream_t st)
+// counter: a word owned by the calling pass: passes of different contexts may run concurrently on one device (emulated ranks on
+// streams), so the tile counter cannot be a per-device static
+bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, unsigned int* counter, cudaStream_t st)
 {
-    if (!counters) return false;
-    using G = TmaGeom<STEP>;
+    if (!counter) return false;
+    using G = TmaGeom;
     if ((((size_t)g.W * 8) & 15) != 0 || ((uintptr_t)g.gb2 & 15) || ((uintptr_t)g.gb3 & 15) || ((uintptr_t)in & 15)) return false;
     CUtensorMap t2, t3, ti;
     if (!tensor_map_2d(g.gb2, g.W, g.H, G::RW, G::RH, &t2) || !tensor_map_2d(g.gb3, g.W, g.H, G::RW, G::RH, &t3) || !tensor_map_2d(in, g.W, g.H, G::RW, G::RH, &ti)) return false;
@@ -605,29 +595,26 @@ bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, co
     static bool configured[64] = {};
     if (hr_once_per_device(configured))
     {
-        cudaFuncSetAttribute(k_refl_atrous_tma<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM);
+        cudaFuncSetAttribute(k_refl_atrous_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM);
         int sms = 132, per_sm = 1;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_atrous_tma<STEP>, 256, G::SMEM);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_atrous_tma, 256, G::SMEM);
         ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);
     }
     const int tiles_x = (P.W + TWR - 1) / TWR, tiles_y = (P.row1 - P.row0 + THR - 1) / THR, n_tiles = tiles_x * tiles_y;
-    unsigned int* ctr = counters + (STEP == 1 ? 0 : STEP == 2 ? 1 : 2);
-    cudaMemsetAsync(ctr, 0, sizeof(unsigned int), st);
+    cudaMemsetAsync(counter, 0, sizeof(unsigned int), st);
     const int grid = ctas[dev] < n_tiles ? ctas[dev] : n_tiles;
-    k_refl_atrous_tma<STEP><<<grid, 256, G::SMEM, st>>>(t2, t3, ti, g, in, tf, P, out, tiles_x, n_tiles, ctr);
+    k_refl_atrous_tma<<<grid, 256, G::SMEM, st>>>(t2, t3, ti, g, in, tf, P, out, tiles_x, n_tiles, counter);
     return true;
 }
 
 } // namespace
 
-// hr_debug_set key 6: 0 = scalar kernel (svgf_reflections.cu), 1 = pixel-pair dense tiles for every step,
-// 2 = pixel pairs, row-interleaved tiles for steps >= 8, 3 (default) = 2 + TMA-staged persistent kernel for step 1,
-// 4 = 2 + TMA-staged persistent kernel for steps 1, 2 and 4.
-// Measured at 4K on an H100 SXM 80 GB (400 W power limit), us per iteration, steps 1 / 2 / 4 / 8: default 123 / 130 / 150 / 160,
-// 4 = 124 / 144 / 149 / 160, scalar kernel 165 / 166 / 178 / 234.  TMA staging loses at step 2, where its raw boxes + planes
-// allow only 2 CTAs per SM (82 KB), and wins at step 1 (74 KB, 3 CTAs per SM): on an H100 SXM 80 GB, 700 W power limit, step 1 takes
-// 113 us with TMA and 118 us with plain staging (2).
+// hr_debug_set key 6: 0 = scalar kernel (svgf_reflections.cu), 2 = pixel pairs with plain staging, row-interleaved tiles for
+// steps >= 8, 3 (default) = 2 + the TMA-staged persistent kernel for step 1.  2 is also what step 1 runs when the TMA set-up
+// fails, and the bit-exact reference of the TMA kernel.  TMA staging wins at step 1 only (74 KB, 3 CTAs per SM; at step 2 its
+// raw boxes + planes allow only 2 CTAs per SM): on an H100 SXM 80 GB, 700 W power limit, step 1 takes 113 us with TMA and
+// 118 us with plain staging (DESIGN.md §8).
 int g_hr_refl_atrous_impl = 3;
 
 // returns false when this variant does not support the configuration (the caller falls back to the scalar kernel)
@@ -639,13 +626,12 @@ bool launch_reflections_atrous_v2(const GBufLevelDev& g, const void* in, const u
     R2Params P { g.W, g.H, 1.44269504f / sigma_depth, -1.44269504f / phi_color, approximate_with_ddgi, row0, row1 };
     const uint2* i2 = (const uint2*)in;
     uint2*       o2 = (uint2*)out;
-    const bool   il = g_hr_refl_atrous_impl >= 2, tma1 = g_hr_refl_atrous_impl >= 3, tma = g_hr_refl_atrous_impl == 4;
     switch (step)
     {
-        case 1: if (!(tma1 && launch_r2_tma<1>(g, i2, tile_flags, P, o2, counters, st))) launch_r2<1>(g, i2, tile_flags, P, o2, st); break;
-        case 2: if (!(tma && launch_r2_tma<2>(g, i2, tile_flags, P, o2, counters, st))) launch_r2<2>(g, i2, tile_flags, P, o2, st); break;
-        case 4: if (!(tma && launch_r2_tma<4>(g, i2, tile_flags, P, o2, counters, st))) launch_r2<4>(g, i2, tile_flags, P, o2, st); break;
-        case 8: if (il) launch_r2s<8>(g, i2, tile_flags, P, o2, st); else launch_r2<8>(g, i2, tile_flags, P, o2, st); break;
+        case 1: if (!(g_hr_refl_atrous_impl == 3 && launch_r2_tma(g, i2, tile_flags, P, o2, counters, st))) launch_r2<1>(g, i2, tile_flags, P, o2, st); break;
+        case 2: launch_r2<2>(g, i2, tile_flags, P, o2, st); break;
+        case 4: launch_r2<4>(g, i2, tile_flags, P, o2, st); break;
+        case 8: launch_r2s<8>(g, i2, tile_flags, P, o2, st); break;
         default: launch_r2s<16>(g, i2, tile_flags, P, o2, st); break;
     }
     return true;

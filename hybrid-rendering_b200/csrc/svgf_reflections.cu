@@ -422,8 +422,6 @@ void launch_atrous_t(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, 
 
 } // namespace
 
-int g_hr_force_peer_temporal = 0; // hr_debug_set(12, 1): run the peer-history variant of K14 on one GPU (overhead A/B of the owner lookups)
-
 void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const void* input, const HistPeers& hist, const FrameConsts& fc, float alpha,
                                  float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st)
 {
@@ -433,7 +431,7 @@ void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& pr
     if (hist.world > 1 && hist.self < hist.world - 1) rot = (row1 - hist.band_end[hist.self] + 7) / 8; // tile rows below this rank's band
     if (rot < 0 || rot >= (int)grid.y) rot = 0;
     ReflTemporalParams P { alpha, moments_alpha, approximate_with_ddgi, row0, row1, rot };
-    if (hist.world > 1 || g_hr_force_peer_temporal) k_refl_temporal<true><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
+    if (hist.world > 1) k_refl_temporal<true><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
     else k_refl_temporal<false><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
 }
 

@@ -521,14 +521,12 @@ HR_API int hr_pass_destroy(hr_pass* pass);
  * Enable with hr_ctx_set_profiling(ctx,1); names/ms arrays of capacity cap; returns count via *n. Synchronises. */
 HR_API int hr_ctx_set_profiling(hr_ctx* ctx, int enabled);
 HR_API int hr_pass_stage_times(hr_pass* pass, const char** names, float* ms, int cap, int* n);
-/* Test / A-B hook.  key 1 = a-trous implementation (0 naive global-memory kernel, 1 shared-memory tiled kernel,
+/* Test hook, process-wide.  key 1 = shadows a-trous implementation (0 naive global-memory kernel, 1 shared-memory tiled kernel,
  * 3 packed fp32x2 pixel-pair kernel = default); key 3 = BVH topology used by the next hr_scene_build / hr_scene_rebuild (0 Karras radix tree,
- * 1 PLOC agglomerative clustering = default); key 4 = run the cooperative (multi-GPU) ray-trace kernel on a single GPU;
- * key 5 = a-trous row-interleaved tiles: 1 = step 8 only (default), 2 = steps 4 and 8, 0 = dense tiles for every step; key 6 = reflections
- * a-trous (0 scalar kernel, 1 packed fp32x2 dense tiles, 2 = packed + row-interleaved tiles for steps >= 8, 3 = 2 + TMA-staged
- * persistent kernel for step 1 = default, 4 = TMA for steps 1, 2, 4); key 8 = reflections a-trous register tuning (CTAs / SM);
- * key 11 = final-output gather: 1 point-to-point = default, 0 per-band broadcasts; key 12 = run the peer-history K14 on one GPU (overhead A/B).  None of them changes a result bit
- * of the visibility masks; keys 1 and 5 select kernels whose outputs agree to the last fp16 bit on the test scenes. */
+ * 1 PLOC agglomerative clustering = default); key 6 = reflections a-trous (0 scalar kernel, 2 packed fp32x2 pixel pairs with plain staging,
+ * 3 = 2 + TMA-staged persistent kernel for step 1 = default).  Any other key, or a value its key does not list, returns
+ * HR_ERR_INVALID_ARG and changes nothing.  None of them changes a result bit of the visibility masks; key 6 values 2 and 3 agree to
+ * the last fp16 bit. */
 HR_API int hr_debug_set(int key, int value);
 /* Number of kernels this library launched since the context was created (bench.py gpu_launches). */
 HR_API uint64_t hr_ctx_launch_count(hr_ctx* ctx);

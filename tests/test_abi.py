@@ -9,6 +9,7 @@ import pytest
 import pyhr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HR_ERR_INVALID_ARG = -1
 
 
 def declared_symbols():
@@ -73,6 +74,22 @@ def test_shard_rows_partition():
             assert all(rows[i][1] == rows[i + 1][0] for i in range(world - 1))
             sizes = [e - b for b, e in rows]
             assert max(sizes) - min(sizes) <= 8 + (-H) % 8  # bands differ by at most one 8-row tile (+ a partial last tile)
+
+
+def test_debug_set_rejects_undefined_keys_and_values():
+    """hr_debug_set touches no device: removed keys and values a key does not define are refused, every defined value is taken"""
+    lib = pyhr.load_product()
+    try:
+        for key in (0, 2, 4, 5, 7, 8, 9, 10, 11, 12, 13):
+            assert lib.hr_debug_set(key, 0) == HR_ERR_INVALID_ARG and lib.hr_debug_set(key, 1) == HR_ERR_INVALID_ARG, key
+        for key, value in ((6, 1), (6, 4), (1, 2), (3, 2), (1, -1), (3, -1), (6, -1), (1, 4), (6, 5)):
+            assert lib.hr_debug_set(key, value) == HR_ERR_INVALID_ARG, (key, value)
+        for key, values in ((1, (0, 1, 3)), (3, (0, 1)), (6, (0, 2, 3))):
+            for value in values:
+                assert lib.hr_debug_set(key, value) == 0, (key, value)
+    finally:
+        for key, default in ((1, 3), (3, 1), (6, 3)):
+            assert lib.hr_debug_set(key, default) == 0
 
 
 def test_init_fails_loudly_without_gpu():

@@ -241,9 +241,8 @@ def test_atrous_tiled_equals_naive_and_oracle_1080p():
     osh = O.ShadowsOracle(W, H, 0)
     f, prev_g = None, O.zero_gbuf_mips(W, H)
     outs = {}
-    for impl in (1, 0, 3, 13, 23):  # 13 / 23 = packed kernel (3) with dense tiles for every step / interleaved rows for steps 4 and 8
-        c.lib.hr_debug_set(1, impl % 10)
-        c.lib.hr_debug_set(5, {13: 0, 23: 2}.get(impl, 1))
+    for impl in (1, 0, 3):
+        c.lib.hr_debug_set(1, impl)
         sh.reset_history()
         f = None
         c.gbuffer_upload(0, pyhr.GBufferHost(W, H))
@@ -258,11 +257,8 @@ def test_atrous_tiled_equals_naive_and_oracle_1080p():
                 osh.render(osc, cur_g, prev_g, f, bn)
                 prev_g = cur_g
         outs[impl] = f16(sh.download(100))
-    c.lib.hr_debug_set(1, 3)  # back to the defaults (process-wide switches)
-    c.lib.hr_debug_set(5, 1)
+    c.lib.hr_debug_set(1, 3)  # back to the default (process-wide switch)
     assert np.array_equal(sh.download(0), osh.mask)
-    # row-interleaved tiles (steps 4, 8) only change which CTA filters which row: same arithmetic per pixel, same bits
-    assert np.array_equal(outs[3], outs[13]) and np.array_equal(outs[3], outs[23])
     ref = O.h2f(osh.final)
     assert rmse(outs[1], outs[0]) <= 2e-4 and np.abs(outs[1] - outs[0]).max() <= 2e-3
     assert rmse(outs[3], outs[0]) <= 2e-4 and np.abs(outs[3] - outs[0]).max() <= 2e-3  # packed fp32x2 kernel
