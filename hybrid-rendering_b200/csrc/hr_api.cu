@@ -6,6 +6,7 @@
 #include <utility>
 #include <cstdarg>
 #include <cstring>
+#include <atomic>
 #include <mutex>
 
 static std::string g_last_error;
@@ -197,6 +198,7 @@ int hr_bluenoise_set_slot(hr_ctx* ctx, int slot, const uint8_t* sr)
 // Scene
 // ---------------------------------------------------------------------------------------------------------------
 static int scene_check_depth(hr_scene* sc);
+static std::atomic<uint64_t> g_scene_serial { 0 }; // hr_scene::serial of the last hr_scene_build, in any context
 
 int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, const uint32_t* indices, size_t n_indices, const hr_instance* instances,
                    size_t n_instances, const hr_material* materials, size_t n_materials, hr_scene** out)
@@ -251,6 +253,7 @@ int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, co
     HR_CUDA(ctx, cudaSetDevice(ctx->device));
     hr_scene* sc = new hr_scene();
     sc->ctx      = ctx;
+    sc->serial   = ++g_scene_serial;
     sc->n_tris   = (uint32_t)n;
     sc->h_vuv    = std::move(vuv);
     sc->h_vtb    = std::move(vtb);

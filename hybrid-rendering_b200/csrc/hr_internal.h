@@ -115,6 +115,8 @@ struct hr_ctx {
 
 struct hr_scene {
     hr_ctx*  ctx     = nullptr;
+    uint64_t serial  = 0;            // process-wide build serial, never 0: identifies the scene where its address cannot (a rebuilt
+                                     // scene may reuse a destroyed one's address; a scene of another context may be set current)
     uint32_t n_tris  = 0;
     uint32_t n_nodes = 0;
     // inputs kept on device for rebuilds
@@ -204,7 +206,7 @@ struct hr_pass {
     // ddgi
     hr_ddgi_uniforms ddgi_u {};
     bool      ddgi_grid_valid = false;
-    const void* ddgi_scene = nullptr;
+    uint64_t  ddgi_scene = 0;                          // hr_scene::serial the grid was built for (0: none)
     float     ddgi_key[4] = { 0, 0, 0, 0 };            // probe_distance, irradiance_oct, depth_oct, rays_per_probe
     int       ddgi_mp = 0;                             // m_ping_pong (ddgi.cpp:103)
     bool      ddgi_first = true;

@@ -144,7 +144,9 @@ typedef struct hr_instance {
 /* Builds the device BVH over all instances' world-space triangles: 63-bit Morton codes + radix sort, then PLOC
  * agglomerative clustering (default) or the Karras radix tree + bottom-up fit (hr_debug_set key 3), collapsed into
  * <= 4-triangle leaves and packed into 64-byte two-child nodes.  Host pointers in; synchronises the context's build
- * stream before returning.  Fails with HR_ERR_UNSUPPORTED when the tree is deeper than the traversal stack (64). */
+ * stream before returning.  Fails with HR_ERR_UNSUPPORTED when the tree is deeper than the traversal stack (64).  Every
+ * built scene gets a new process-wide serial number; a DDGI pass re-initialises its probe grid when it next renders a scene
+ * with another serial, even one allocated at a destroyed scene's address. */
 HR_API int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, const uint32_t* indices, size_t n_indices,
                           const hr_instance* instances, size_t n_instances, const hr_material* materials, size_t n_materials,
                           hr_scene** out);
@@ -369,8 +371,13 @@ HR_API void hr_ddgi_default_params(hr_ddgi_params* p);
 HR_API int  hr_ddgi_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** out); /* ddgi.cpp:60-76 */
 /* render(), ddgi.cpp:89-104.  random_orientation: column-major mat4 (the reference draws it from std::mt19937 seeded by
  * std::random_device, ddgi.cpp:73,788 — non-deterministic; the caller supplies it).  The probe grid is (re)initialised from
- * the current scene's bounds when the scene or probe_distance / oct sizes / rays_per_probe change (ddgi.cpp:150-169). */
+ * the current scene's bounds on the first render, when the current scene is another hr_scene_build's (even at a reused address),
+ * when probe_distance / irradiance_oct_size / depth_oct_size / rays_per_probe change, and after a failed initialisation
+ * (ddgi.cpp:150-169).  A re-initialised grid starts like the first frame: zero atlases, no hysteresis, no infinite bounce.  The
+ * other parameters are applied every frame.  Out-of-range parameters return HR_ERR_INVALID_ARG and change nothing; a grid of
+ * more than 2^20 probes returns HR_ERR_UNSUPPORTED and leaves the pass without a grid (the next render initialises one). */
 HR_API int hr_ddgi_render(hr_pass* pass, const hr_frame* frame, const hr_ddgi_params* params, const float* random_orientation16, void* stream);
+/* The uniforms of the current grid; HR_ERR_NOT_READY before the first render and after a failed grid initialisation. */
 HR_API int hr_ddgi_get_uniforms(hr_pass* pass, hr_ddgi_uniforms* out);
 
 /* ------------------------------------------------------------------------------------------------

@@ -399,6 +399,14 @@ def gbuffer_render(ss: "ShadingScene", frame, W, H, out=None):
     return g
 
 
+def ddgi_update_properties(u, params):
+    """update_properties_ubo (ddgi.cpp:738-763): the parameters that do not shape the grid, applied every frame"""
+    u.max_distance = params.probe_distance * 1.5
+    u.depth_sharpness, u.hysteresis, u.normal_bias = params.depth_sharpness, params.hysteresis, params.normal_bias
+    u.energy_preservation = params.recursive_energy_preservation
+    u.visibility_test = params.visibility_test
+
+
 def ddgi_uniforms_from(params, bounds_min, bounds_max):
     """initialize_probe_grid + update_properties_ubo (ddgi.cpp:150-169, :738-763)"""
     u = pyhr.hr_ddgi_uniforms()
@@ -408,20 +416,20 @@ def ddgi_uniforms_from(params, bounds_min, bounds_max):
         u.grid_start_position[a] = float(bounds_min[a])
         u.grid_step[a] = params.probe_distance
     cx, cy, cz = u.probe_counts[0], u.probe_counts[1], u.probe_counts[2]
-    u.max_distance = params.probe_distance * 1.5
-    u.depth_sharpness, u.hysteresis, u.normal_bias = params.depth_sharpness, params.hysteresis, params.normal_bias
-    u.energy_preservation = params.recursive_energy_preservation
     u.irradiance_probe_side_length, u.depth_probe_side_length = params.irradiance_oct_size, params.depth_oct_size
     u.irradiance_texture_width = (params.irradiance_oct_size + 2) * cx * cy + 2
     u.irradiance_texture_height = (params.irradiance_oct_size + 2) * cz + 2
     u.depth_texture_width = (params.depth_oct_size + 2) * cx * cy + 2
     u.depth_texture_height = (params.depth_oct_size + 2) * cz + 2
-    u.rays_per_probe, u.visibility_test = params.rays_per_probe, params.visibility_test
+    u.rays_per_probe = params.rays_per_probe
+    ddgi_update_properties(u, params)
     return u
 
 
 class DDGIOracle:
-    """DDGI::render, src/ddgi.cpp:89-104"""
+    """DDGI::render, src/ddgi.cpp:89-104.  The grid is fixed at construction: a change of probe_distance, the oct sizes or
+    rays_per_probe (which re-initialises the device's grid) needs a new DDGIOracle.  The other parameters are read from
+    `params` every frame, like the device does."""
 
     def __init__(self, W0, H0, scale, params, bounds_min, bounds_max):
         self.W, self.H = pass_size(W0, H0, scale)
@@ -437,7 +445,12 @@ class DDGIOracle:
         self.sample = np.zeros((self.H, self.W, 4), np.uint16)
         self.mp, self.first = 0, True
 
+    def update_properties(self):
+        """refresh the uniforms from `params` (update_properties_ubo); render() does this first"""
+        ddgi_update_properties(self.u, self.params)
+
     def render(self, ss: ShadingScene, cur: GBufMips, frame, rot16):
+        self.update_properties()
         L, P, u, mp = lib(), self.params, self.u, self.mp
         sky = np.array(P.sky_color[:], np.float32)
         rot = np.ascontiguousarray(rot16, np.float32)

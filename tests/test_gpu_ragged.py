@@ -176,13 +176,32 @@ def test_ao_blur_radius(blur_radius):
 
 
 # ---------------------------------------------------------------------------------------------- DDGI + reflections
+def check_ddgi(i, dd, odd, w):
+    """every DDGI output against the oracle: uniforms bytes and ray directions / hit distances exact, images under `close`"""
+    assert bytes(dd.uniforms()) == bytes(odd.u), f"frame {i}: DDGIUniforms differ"
+    dird_c = dd.download(1).view(np.uint16)
+    assert np.array_equal(dird_c, odd.dirdepth.reshape(dird_c.shape)), f"frame {i}: probe ray direction / hit distance not exact"
+    close(f16(dd.download(0)), O.h2f(odd.radiance).reshape(-1, odd.u.rays_per_probe, 4), f"frame {i} ddgi radiance", 2e-3, 0.05)
+    close(f16(dd.download(2)), O.h2f(odd.cur_irr), f"frame {i} irradiance atlas")
+    close(f16(dd.download(3)), O.h2f(odd.cur_dep), f"frame {i} depth atlas", 2e-3, 0.05)
+    close(f16(dd.download(4)), O.h2f(odd.sample), f"frame {i} ddgi sample")
+    w.add("ddgi irradiance", f16(dd.download(2)), O.h2f(odd.cur_irr))
+    w.add("ddgi sample", f16(dd.download(4)), O.h2f(odd.sample))
+
+
 def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0, cam=CAM_SHADOWS_TEST,
-                light=None):
-    """test_gpu_gi_refl.run at any size and scale (DDGI sampled at the reflections' scale), fed by the device G-buffer producer"""
-    sc = pyhr.SynthScene(scene, tris)
+                light=None, ddgi_params=None, lut=None, ddgi_hook=None):
+    """test_gpu_gi_refl.run at any size and scale (DDGI sampled at the reflections' scale), fed by the device G-buffer producer.
+    ddgi_params: overrides of the DDGI parameter block; lut: a BRDF LUT set on the context and the oracle (the reflections' IBL
+    specular term, as in test_deferred); ddgi_hook(i, f, rot, dd, odd, fresh) runs before frame i's DDGI render and returns the
+    DDGI oracle to go on with (fresh() makes a new one from dd.params: a re-initialised grid).  scene: a SynthScene kind, or an
+    object with SynthScene's interface"""
+    sc = pyhr.SynthScene(scene, tris) if isinstance(scene, int) else scene
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
     ctx = new_context(sc, W, H)
+    if lut is not None:
+        ctx.set_brdf_lut(lut)
     mn, mx = sc.bounds()
     dd = pyhr.DDGIPass(ctx, W, H, scale) if with_ddgi else None
     rf = pyhr.ReflectionsPass(ctx, W, H, scale)
@@ -193,8 +212,14 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
     if dd:
         dd.params.probe_distance = 4.0 if scene == pyhr.SCENE_SHADOWS_TEST else 12.0
         dd.params.normal_bias = 1.0
-        odd = O.DDGIOracle(W, H, scale, dd.params, mn, mx)
+        set_params([dd.params], ddgi_params)  # ... and so does the DDGI oracle
+
+        def fresh():
+            return O.DDGIOracle(W, H, scale, dd.params, mn, mx)
+        odd = fresh()
     orf = O.ReflectionsOracle(W, H, scale, rf.params)
+    if lut is not None:
+        orf.brdf_lut = lut
     w = Worst(case)
     prev_g = O.zero_gbuf_mips(W, H)
     for i, f in frames(W, H, n, pan_from, vertical, cam, light):
@@ -203,18 +228,11 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
         same_gbuffer(ctx, f, cur_g, W, H)
         if dd:
             rot = pyhr.rotation_matrix(0.7 + 1.3 * i, (0.3, 1.0, -0.5))
+            if ddgi_hook:
+                odd = ddgi_hook(i, f, rot, dd, odd, fresh)
             dd.render(f, rot)
             odd.render(ss, cur_g, f, rot)
-            if i == 0:
-                assert bytes(dd.uniforms()) == bytes(odd.u), "DDGIUniforms differ"
-            dird_c = dd.download(1).view(np.uint16)
-            assert np.array_equal(dird_c, odd.dirdepth.reshape(dird_c.shape)), f"frame {i}: probe ray direction / hit distance not exact"
-            close(f16(dd.download(0)), O.h2f(odd.radiance).reshape(-1, odd.u.rays_per_probe, 4), f"frame {i} ddgi radiance", 2e-3, 0.05)
-            close(f16(dd.download(2)), O.h2f(odd.cur_irr), f"frame {i} irradiance atlas")
-            close(f16(dd.download(3)), O.h2f(odd.cur_dep), f"frame {i} depth atlas", 2e-3, 0.05)
-            close(f16(dd.download(4)), O.h2f(odd.sample), f"frame {i} ddgi sample")
-            w.add("ddgi irradiance", f16(dd.download(2)), O.h2f(odd.cur_irr))
-            w.add("ddgi sample", f16(dd.download(4)), O.h2f(odd.sample))
+            check_ddgi(i, dd, odd, w)
         rf.render(f, dd)
         orf.render(ss, cur_g, prev_g, f, bn, odd)
         prev_g = cur_g
