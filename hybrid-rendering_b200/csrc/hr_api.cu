@@ -55,13 +55,18 @@ static FrameConsts make_consts(const hr_frame* f, const hr_pass* p)
     return c;
 }
 
+// extent of mip `mip` of an image `v` texels wide (or high): halved per level, never below 1
+static int mip_extent(int v, int mip)
+{
+    for (int m = 0; m < mip; m++) v = v / 2 > 0 ? v / 2 : 1;
+    return v;
+}
+
 static GBufLevelDev level_view(const hr_ctx* ctx, int slot, int mip)
 {
     GBufLevelDev l;
-    int          w = ctx->gb_w, h = ctx->gb_h;
-    for (int m = 0; m < mip; m++) { w = w / 2 > 0 ? w / 2 : 1; h = h / 2 > 0 ? h / 2 : 1; }
-    l.W     = w;
-    l.H     = h;
+    l.W     = mip_extent(ctx->gb_w, mip);
+    l.H     = mip_extent(ctx->gb_h, mip);
     l.gb1   = (const uint32_t*)ctx->slot[slot].gb1[mip];
     l.gb2   = (const uint2*)ctx->slot[slot].gb2[mip];
     l.gb3   = (const uint2*)ctx->slot[slot].gb3[mip];
@@ -477,10 +482,9 @@ int hr_gbuffer_create(hr_ctx* ctx, int width, int height)
     ctx->gb_h = height;
     for (int s = 0; s < 2; s++)
     {
-        int w = width, h = height;
         for (int m = 0; m < HR_MAX_MIPS; m++)
         {
-            const size_t px = (size_t)w * h;
+            const size_t px = (size_t)mip_extent(width, m) * mip_extent(height, m);
             HR_CUDA(ctx, cudaMalloc(&ctx->slot[s].gb1[m], px * 4));
             HR_CUDA(ctx, cudaMalloc(&ctx->slot[s].gb2[m], px * 8));
             HR_CUDA(ctx, cudaMalloc(&ctx->slot[s].gb3[m], px * 8));
@@ -489,8 +493,6 @@ int hr_gbuffer_create(hr_ctx* ctx, int width, int height)
             HR_CUDA(ctx, cudaMemset(ctx->slot[s].gb2[m], 0, px * 8));
             HR_CUDA(ctx, cudaMemset(ctx->slot[s].gb3[m], 0, px * 8));
             HR_CUDA(ctx, cudaMemset(ctx->slot[s].depth[m], 0, px * 4));
-            w = w / 2 > 0 ? w / 2 : 1;
-            h = h / 2 > 0 ? h / 2 : 1;
         }
         ctx->owned_mip0[s][0] = ctx->slot[s].gb1[0];
         ctx->owned_mip0[s][1] = ctx->slot[s].gb2[0];
@@ -501,18 +503,24 @@ int hr_gbuffer_create(hr_ctx* ctx, int width, int height)
     return HR_OK;
 }
 
+// Point slot `slot` at its library-owned mip-0 storage (the slot may have been bound zero-copy before).
+static GBufSlot& use_owned_mip0(hr_ctx* ctx, int slot)
+{
+    GBufSlot& s = ctx->slot[slot];
+    s.gb1[0]   = ctx->owned_mip0[slot][0];
+    s.gb2[0]   = ctx->owned_mip0[slot][1];
+    s.gb3[0]   = ctx->owned_mip0[slot][2];
+    s.depth[0] = (float*)ctx->owned_mip0[slot][3];
+    return s;
+}
+
 static int gbuffer_copy_in(hr_ctx* ctx, int slot, const hr_gbuffer_desc* src, cudaMemcpyKind kind, cudaStream_t st)
 {
     HR_REQUIRE(ctx, ctx && src && (slot == 0 || slot == 1), HR_ERR_INVALID_ARG, "hr_gbuffer_upload: bad argument");
     HR_REQUIRE(ctx, ctx->gb_w > 0, HR_ERR_NOT_READY, "hr_gbuffer_upload: call hr_gbuffer_create first");
     HR_REQUIRE(ctx, src->width == ctx->gb_w && src->height == ctx->gb_h, HR_ERR_INVALID_ARG, "hr_gbuffer_upload: size mismatch");
     HR_REQUIRE(ctx, src->gb2 && src->gb3 && src->depth, HR_ERR_INVALID_ARG, "hr_gbuffer_upload: gb2/gb3/depth are required");
-    GBufSlot& s = ctx->slot[slot];
-    // restore library-owned mip0 storage if the slot was bound zero-copy before
-    s.gb1[0]   = ctx->owned_mip0[slot][0];
-    s.gb2[0]   = ctx->owned_mip0[slot][1];
-    s.gb3[0]   = ctx->owned_mip0[slot][2];
-    s.depth[0] = (float*)ctx->owned_mip0[slot][3];
+    GBufSlot&    s  = use_owned_mip0(ctx, slot);
     const size_t px = (size_t)ctx->gb_w * ctx->gb_h;
     if (src->gb1) HR_CUDA(ctx, cudaMemcpyAsync(s.gb1[0], src->gb1, px * 4, kind, st));
     HR_CUDA(ctx, cudaMemcpyAsync(s.gb2[0], src->gb2, px * 8, kind, st));
@@ -530,17 +538,14 @@ int hr_gbuffer_copy_from_device(hr_ctx* ctx, int slot, const hr_gbuffer_desc* de
 // renders, so the copy goes to a third surface on the library's upload stream; commit swaps that surface with the slot's
 // storage.  The storage handed back by the swap was last read by renders already enqueued on `stream`: an event recorded
 // there gates the next staged upload.
-int hr_gbuffer_stage_upload(hr_ctx* ctx, const hr_gbuffer_desc* host)
+// The staging surface, the upload stream and its events are created on the first staged frame; the upload stream then waits
+// until the storage that the last commit handed back is no longer read.
+static int staging_begin(hr_ctx* ctx)
 {
-    HR_REQUIRE(ctx, ctx && host, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: bad argument");
-    HR_REQUIRE(ctx, ctx->gb_w > 0, HR_ERR_NOT_READY, "hr_gbuffer_stage_upload: call hr_gbuffer_create first");
-    HR_REQUIRE(ctx, host->width == ctx->gb_w && host->height == ctx->gb_h, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: size mismatch");
-    HR_REQUIRE(ctx, host->gb2 && host->gb3 && host->depth, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: gb2/gb3/depth are required");
-    HR_REQUIRE(ctx, !ctx->staged_pending, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: a staged frame is already waiting for hr_gbuffer_commit_staged");
     HR_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t px = (size_t)ctx->gb_w * ctx->gb_h;
     if (!ctx->upload_stream)
     {
+        const size_t px = (size_t)ctx->gb_w * ctx->gb_h;
         HR_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->upload_stream, cudaStreamNonBlocking));
         HR_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_staged, cudaEventDisableTiming));
         HR_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_storage_free, cudaEventDisableTiming));
@@ -552,6 +557,19 @@ int hr_gbuffer_stage_upload(hr_ctx* ctx, const hr_gbuffer_desc* host)
         }
     }
     if (ctx->storage_free_recorded) HR_CUDA(ctx, cudaStreamWaitEvent(ctx->upload_stream, ctx->ev_storage_free, 0));
+    return HR_OK;
+}
+
+int hr_gbuffer_stage_upload(hr_ctx* ctx, const hr_gbuffer_desc* host)
+{
+    HR_REQUIRE(ctx, ctx && host, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: bad argument");
+    HR_REQUIRE(ctx, ctx->gb_w > 0, HR_ERR_NOT_READY, "hr_gbuffer_stage_upload: call hr_gbuffer_create first");
+    HR_REQUIRE(ctx, host->width == ctx->gb_w && host->height == ctx->gb_h, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: size mismatch");
+    HR_REQUIRE(ctx, host->gb2 && host->gb3 && host->depth, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: gb2/gb3/depth are required");
+    HR_REQUIRE(ctx, !ctx->staged_pending, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_upload: a staged frame is already waiting for hr_gbuffer_commit_staged");
+    int rc = staging_begin(ctx);
+    if (rc != HR_OK) return rc;
+    const size_t px = (size_t)ctx->gb_w * ctx->gb_h;
     if (host->gb1) HR_CUDA(ctx, cudaMemcpyAsync(ctx->staging_mip0[0], host->gb1, px * 4, cudaMemcpyHostToDevice, ctx->upload_stream));
     HR_CUDA(ctx, cudaMemcpyAsync(ctx->staging_mip0[1], host->gb2, px * 8, cudaMemcpyHostToDevice, ctx->upload_stream));
     HR_CUDA(ctx, cudaMemcpyAsync(ctx->staging_mip0[2], host->gb3, px * 8, cudaMemcpyHostToDevice, ctx->upload_stream));
@@ -569,21 +587,8 @@ int hr_gbuffer_stage_render(hr_ctx* ctx, const hr_frame* frame)
     HR_REQUIRE(ctx, ctx->gb_w > 0, HR_ERR_NOT_READY, "hr_gbuffer_stage_render: call hr_gbuffer_create first");
     HR_REQUIRE(ctx, ctx->scene && ctx->scene->d_materials, HR_ERR_NOT_READY, "hr_gbuffer_stage_render: no current scene with materials (hr_scene_build)");
     HR_REQUIRE(ctx, !ctx->staged_pending, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_render: a staged frame is already waiting for hr_gbuffer_commit_staged");
-    HR_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t px = (size_t)ctx->gb_w * ctx->gb_h;
-    if (!ctx->upload_stream)
-    {
-        HR_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->upload_stream, cudaStreamNonBlocking));
-        HR_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_staged, cudaEventDisableTiming));
-        HR_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_storage_free, cudaEventDisableTiming));
-        const size_t bytes[4] = { px * 4, px * 8, px * 8, px * 4 };
-        for (int k = 0; k < 4; k++)
-        {
-            HR_CUDA(ctx, cudaMalloc(&ctx->staging_mip0[k], bytes[k]));
-            HR_CUDA(ctx, cudaMemset(ctx->staging_mip0[k], 0, bytes[k]));
-        }
-    }
-    if (ctx->storage_free_recorded) HR_CUDA(ctx, cudaStreamWaitEvent(ctx->upload_stream, ctx->ev_storage_free, 0));
+    int rc = staging_begin(ctx);
+    if (rc != HR_OK) return rc;
     launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, 0, ctx->gb_h, 0, 1, ctx->staging_mip0[0], ctx->staging_mip0[1], ctx->staging_mip0[2],
                           (float*)ctx->staging_mip0[3], ctx->gbuf_ray_ctr, ctx->upload_stream);
     ctx->launches++;
@@ -602,12 +607,8 @@ int hr_gbuffer_commit_staged(hr_ctx* ctx, int slot, void* stream)
     HR_CUDA(ctx, cudaEventRecord(ctx->ev_storage_free, st));
     ctx->storage_free_recorded = true;
     HR_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_staged, 0));
-    GBufSlot& s = ctx->slot[slot];
     for (int k = 0; k < 4; k++) std::swap(ctx->owned_mip0[slot][k], ctx->staging_mip0[k]);
-    s.gb1[0]   = ctx->owned_mip0[slot][0];
-    s.gb2[0]   = ctx->owned_mip0[slot][1];
-    s.gb3[0]   = ctx->owned_mip0[slot][2];
-    s.depth[0] = (float*)ctx->owned_mip0[slot][3];
+    GBufSlot& s = use_owned_mip0(ctx, slot);
     ctx->staged_pending = false;
     return hr_launch_build_mips(ctx, s, ctx->gb_w, ctx->gb_h, st);
 }
@@ -634,11 +635,7 @@ int hr_gbuffer_render(hr_ctx* ctx, int slot, const hr_frame* frame, int row0, in
     if (row1 <= 0) { row0 = 0; row1 = ctx->gb_h; }
     HR_REQUIRE(ctx, row0 >= 0 && row1 > row0 && row1 <= ctx->gb_h && row0 % 8 == 0 && (row1 % 8 == 0 || row1 == ctx->gb_h), HR_ERR_INVALID_ARG,
                "hr_gbuffer_render: rows must be multiples of 8 (or end at the image height)");
-    GBufSlot& s = ctx->slot[slot];
-    s.gb1[0]   = ctx->owned_mip0[slot][0]; // library-owned storage (the slot may have been bound zero-copy before)
-    s.gb2[0]   = ctx->owned_mip0[slot][1];
-    s.gb3[0]   = ctx->owned_mip0[slot][2];
-    s.depth[0] = (float*)ctx->owned_mip0[slot][3];
+    GBufSlot& s = use_owned_mip0(ctx, slot);
     launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, row0, row1, 0, 1, s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr, (cudaStream_t)stream);
     ctx->launches++;
     HR_CHECK_LAUNCH(ctx);
@@ -653,11 +650,7 @@ int hr_gbuffer_render_sharded(hr_ctx* ctx, int slot, const hr_frame* frame, int 
     if (ctx->world <= 1) return hr_gbuffer_render(ctx, slot, frame, 0, 0, stream);
     HR_REQUIRE(ctx, ctx->gb_w > 0, HR_ERR_NOT_READY, "hr_gbuffer_render_sharded: call hr_gbuffer_create first");
     HR_REQUIRE(ctx, ctx->scene && ctx->scene->d_materials, HR_ERR_NOT_READY, "hr_gbuffer_render_sharded: no current scene with materials (hr_scene_build)");
-    GBufSlot& s = ctx->slot[slot];
-    s.gb1[0]   = ctx->owned_mip0[slot][0];
-    s.gb2[0]   = ctx->owned_mip0[slot][1];
-    s.gb3[0]   = ctx->owned_mip0[slot][2];
-    s.depth[0] = (float*)ctx->owned_mip0[slot][3];
+    GBufSlot& s = use_owned_mip0(ctx, slot);
     int b0, b1, r0, r1;
     hr_band(ctx, ctx->gb_h, &b0, &b1);
     hr_extend(b0, b1, round_up8(halo_rows), ctx->gb_h, &r0, &r1);
@@ -710,28 +703,32 @@ static int pass_alloc(hr_pass* p, T*& ptr, size_t count, int fill_byte = 0)
     return HR_OK;
 }
 
+// The images of a pass being created: after the first failed allocation the later ones are skipped and `rc` keeps the error.
+struct PassAllocs {
+    hr_pass* p;
+    int      rc = HR_OK;
+    template <typename T>
+    void operator()(T*& ptr, size_t count, int fill_byte = 0) { if (rc == HR_OK) rc = pass_alloc(p, ptr, count, fill_byte); }
+};
+
 // multi-GPU ray-trace sharing (shard.cu): second ray-mask image (frame parity), cost tables, device-side row partition
-static int pass_alloc_rt_share(hr_pass* p)
+static void pass_alloc_rt_share(PassAllocs& A)
 {
+    hr_pass*     p  = A.p;
     const size_t mw = (p->W + 7) / 8, mh = (p->H + 3) / 4;
-    int          rc;
     p->mask_pp[0] = p->mask;
-    if ((rc = pass_alloc(p, p->mask_pp[1], mw * mh)) != HR_OK) return rc;
-    if ((rc = pass_alloc(p, p->rt_cost_all, 2 * mh)) != HR_OK) return rc;
-    if ((rc = pass_alloc(p, p->rt_cost_acc, mh)) != HR_OK) return rc;
-    if ((rc = pass_alloc(p, p->rt_bounds, (size_t)HR_MAX_RANKS + 4)) != HR_OK) return rc; // + job counter, push-blocks-done counter
-    return HR_OK;
+    A(p->mask_pp[1], mw * mh);
+    A(p->rt_cost_all, 2 * mh);
+    A(p->rt_cost_acc, mh);
+    A(p->rt_bounds, (size_t)HR_MAX_RANKS + 4); // + job counter, push-blocks-done counter
 }
 
-static void set_view(hr_pass* p, int which, void* ptr, int w, int h, int fmt)
-{
-    p->out_view[which].p   = ptr;
-    p->out_view[which].w   = w;
-    p->out_view[which].h   = h;
-    p->out_view[which].fmt = fmt;
-}
+static void set_view(hr_pass* p, int which, void* ptr, int w, int h, int fmt) { p->out_view[which] = { ptr, w, h, fmt }; }
 
-static int pass_common_create(hr_ctx* ctx, int width, int height, int scale, int kind, hr_pass** out)
+// A pass of `kind` at (width, height) / 2^scale; `alloc` allocates its images through the PassAllocs it is given.  If an
+// allocation fails the pass is destroyed and *out is null.
+template <typename Alloc>
+static int pass_create(hr_ctx* ctx, int width, int height, int scale, int kind, hr_pass** out, Alloc alloc)
 {
     HR_REQUIRE(ctx, ctx && out && width > 0 && height > 0 && scale >= 0 && scale < HR_MAX_MIPS, HR_ERR_INVALID_ARG, "pass create: bad argument");
     HR_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -741,14 +738,15 @@ static int pass_common_create(hr_ctx* ctx, int width, int height, int scale, int
     p->W0      = width;
     p->H0      = height;
     p->scale   = scale;
-    int w = width, h = height;
-    for (int m = 0; m < scale; m++) { w = w / 2 > 0 ? w / 2 : 1; h = h / 2 > 0 ? h / 2 : 1; } // = swapchain / 2^scale, ray_traced_shadows.cpp:78-83
-    p->W = w;
-    p->H = h;
+    p->W       = mip_extent(width, scale); // = swapchain / 2^scale, ray_traced_shadows.cpp:78-83
+    p->H       = mip_extent(height, scale);
     const size_t ctr_bytes = sizeof(unsigned long long) * 2 * HR_RAY_CTR_SLOTS * HR_RAY_CTR_STRIDE;
     if (cudaMalloc((void**)&p->ray_ctr, ctr_bytes) != cudaSuccess) { delete p; hr_set_error(ctx, "pass create: out of memory"); return HR_ERR_OUT_OF_MEMORY; }
     cudaMemset(p->ray_ctr, 0, ctr_bytes);
     p->allocs.push_back(p->ray_ctr);
+    PassAllocs A { p };
+    alloc(A);
+    if (A.rc != HR_OK) { hr_pass_destroy(p); *out = nullptr; return A.rc; }
     *out = p;
     return HR_OK;
 }
@@ -764,24 +762,152 @@ static int atrous_halo_rows(int radius, int iterations)
     return round_up8((int)(h > (1 << 20) ? (1 << 20) : h) + 1);
 }
 
+// The whole plan: rows beyond its band that a sharded rank's temporal / a-trous / horizontal-blur stages compute (`denoise`), that its
+// band-local ray trace covers for them (`ray_trace`), and that the AO vertical blur computes (`vblur`: band + 8, the upsample reads one
+// coarse row beyond the band; it reads +- blur_radius rows of the horizontal blur, which is pointwise in y over the temporal output).
+struct HaloPlan { int denoise, ray_trace, vblur; };
+static_assert(PASS_SHADOWS == HR_PASS_KIND_SHADOWS && PASS_AO == HR_PASS_KIND_AO && PASS_REFLECTIONS == HR_PASS_KIND_REFLECTIONS, "pass kinds");
+static HaloPlan halo_plan(int kind, int radius, int filter_iterations, int blur_radius)
+{
+    HaloPlan h;
+    h.vblur     = kind == PASS_AO ? 8 : 0;
+    h.denoise   = kind == PASS_AO ? h.vblur + round_up8(blur_radius) : atrous_halo_rows(radius, filter_iterations);
+    h.ray_trace = h.denoise + 8; // 17x17 statistics of the temporal stage
+    return h;
+}
+
 // The plan above as a pure query (no context, no GPU): which rows beyond its band a sharded rank computes.  Tests restate the plan on
-// the CPU oracle with these numbers (tests/test_sharding_cpu.py) and the render functions use the same two helpers.
+// the CPU oracle with these numbers (tests/test_sharding_cpu.py); the render functions take their halos from halo_plan too.
 int hr_shard_halo_rows(int pass_kind, int radius, int filter_iterations, int blur_radius, int* denoise_halo, int* ray_trace_halo)
 {
     if (!denoise_halo || !ray_trace_halo || radius < 0 || filter_iterations < 0 || blur_radius < 0) return HR_ERR_INVALID_ARG;
-    switch (pass_kind)
+    if (pass_kind != HR_PASS_KIND_SHADOWS && pass_kind != HR_PASS_KIND_AO && pass_kind != HR_PASS_KIND_REFLECTIONS) return HR_ERR_INVALID_ARG;
+    const HaloPlan h = halo_plan(pass_kind, radius, filter_iterations, blur_radius);
+    *denoise_halo    = h.denoise;
+    *ray_trace_halo  = h.ray_trace;
+    return HR_OK;
+}
+
+// ---- the frame protocol of the shadows, AO and reflections renders ------------------------------------------------
+// One render: the rows its stages compute, its frame tick and its final output.  frame_begin / frame_end are the parts the three
+// renders share; the clears, the history waits and the gathers between them are per pass.
+struct PassFrame {
+    cudaStream_t st;
+    int          pp, epoch;
+    bool         no_history;        // first frame after creation / hr_pass_reset_history: the reprojection reads no history
+    bool         signalled = false; // this frame's history tick is published (frame_signal)
+    int          b0, b1;            // owned band (hr_band)
+    int          rt0, rt1, rt_halo; // band-local ray trace: band +- rt_halo
+    int          row0, row1;        // temporal / a-trous / horizontal blur
+    int          v0, v1;            // AO vertical blur
+    int          up0, up1;          // full-resolution rows of the upsample
+    hr_pass::Img final;             // output 100
+};
+
+static int frame_begin(hr_pass* p, const hr_frame* f, bool denoise, const HaloPlan& plan, cudaStream_t st, PassFrame* fr)
+{
+    hr_ctx*        ctx = p->ctx;
+    const HaloPlan h   = ctx->world > 1 && denoise ? plan : HaloPlan { 0, 0, 0 };
+    fr->st = st;
+    fr->pp = f->ping_pong;
+    hr_band(ctx, p->H, &fr->b0, &fr->b1);
+    hr_extend(fr->b0, fr->b1, h.ray_trace, p->H, &fr->rt0, &fr->rt1);
+    hr_extend(fr->b0, fr->b1, h.denoise, p->H, &fr->row0, &fr->row1);
+    hr_extend(fr->b0, fr->b1, h.vblur, p->H, &fr->v0, &fr->v1);
+    fr->rt_halo     = h.ray_trace;
+    fr->up0         = fr->b0 << p->scale;
+    fr->up1         = fr->b1 >= p->H ? p->H0 : (fr->b1 << p->scale);
+    p->last_rows[0] = fr->row0;
+    p->last_rows[1] = fr->row1;
+    timer_begin(p, st);
+    int rc = hr_peer_link_ipc(p, st); // first sharded render: map the peers' history / ray-trace images (collective, shard.cu)
+    if (rc != HR_OK) return rc;
+    fr->epoch = ++p->epoch;
+    p->n_renders++;
+    fr->no_history = p->first;
+    return HR_OK;
+}
+
+// Publish this frame's history tick: every history image the next frame's reprojection reads from this rank is complete.
+static int frame_signal(hr_pass* p, PassFrame& fr)
+{
+    fr.signalled = true;
+    return hr_peer_signal(p, 0, fr.epoch, fr.st);
+}
+
+static int frame_end(hr_pass* p, PassFrame& fr)
+{
+    if (!fr.signalled)
     {
-        case HR_PASS_KIND_SHADOWS:
-        case HR_PASS_KIND_REFLECTIONS:
-            *denoise_halo   = atrous_halo_rows(radius, filter_iterations);
-            *ray_trace_halo = *denoise_halo + 8; // 17x17 statistics of the temporal stage
-            return HR_OK;
-        case HR_PASS_KIND_AO:
-            *denoise_halo   = 8 + round_up8(blur_radius); // temporal / horizontal blur rows; the vertical blur erodes blur_radius of them
-            *ray_trace_halo = *denoise_halo + 8;
-            return HR_OK;
-        default: return HR_ERR_INVALID_ARG;
+        const int rc = frame_signal(p, fr);
+        if (rc != HR_OK) return rc;
     }
+    p->out_view[100] = fr.final;
+    HR_CHECK_LAUNCH(p->ctx);
+    return HR_OK;
+}
+
+static const char* const atrous_stage_names[8] = { "A-Trous 0", "A-Trous 1", "A-Trous 2", "A-Trous 3", "A-Trous 4", "A-Trous 5", "A-Trous 6", "A-Trous 7" };
+
+// ---- stages shared by shadows and AO -------------------------------------------------------------------------------
+static_assert((int)HR_SHADOWS_OUT_RAY_TRACE == (int)HR_AO_OUT_RAY_TRACE && (int)HR_SHADOWS_OUT_UPSAMPLE == (int)HR_AO_OUT_UPSAMPLE, "shared output slots");
+
+// ray_trace (ray_traced_shadows.cpp:972-1011, ray_traced_ao.cpp:864-903): K1 (p0 = bias) or K7 (p0 = ray length, p1 = bias) into
+// the mask image, or with spp > 1 into the count image, then the wait for last frame's history if the temporal stage reads it.
+// Linked to peers (spp = 1): this rank traces its cost-balanced share of the WHOLE image and stores the mask words into every
+// rank's mask image (no halo re-trace); otherwise its band +- the ray-trace halo into its own image.
+static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const FrameConsts& fc, float p0, float p1, int spp, bool denoise, uint32_t** mask_out,
+                      bool* shared_out)
+{
+    hr_ctx*      ctx    = p->ctx;
+    const int    parity = fr.epoch & 1;
+    const BvhDev bvh    = hr_bvh_view(ctx->scene);
+    RtShare      rts;
+    const bool   shared = spp == 1 && hr_rt_share(p, parity, &rts);
+    uint32_t*    mask   = shared ? p->mask_pp[parity] : p->mask;
+    int          rc;
+    if (shared)
+    {
+        launch_ray_trace_mask_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, rts, fr.st);
+        ctx->launches++;
+        if ((rc = hr_rt_share_finish(p, parity, fr.epoch, fr.st)) != HR_OK) return rc;
+        timer_mark(p, "Ray Trace", fr.st);
+        // every rank's share of this frame's mask (and cost table) has arrived and, when the temporal stage reads it, last frame's
+        // history is complete: this wait also covers the history tick, so the temporal stage does not wait on it again
+        if ((rc = hr_rt_wait_partition(p, parity, fr.epoch, (denoise && !fr.no_history) ? fr.epoch - 1 : 0, fr.st)) != HR_OK) return rc;
+        timer_mark(p, "Mask Exchange Wait", fr.st);
+    }
+    else
+    {
+        if (spp > 1)
+        { // SURVEY.md §8d: spp rays per pixel into an 8-bit count image (allocated on first use)
+            if (!p->count && (rc = pass_alloc(p, p->count, (size_t)p->W * p->H)) != HR_OK) return rc;
+            launch_ray_trace_count(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), p->count, spp, fr.rt0, fr.rt1, fr.st);
+        }
+        else launch_ray_trace_mask(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, mask, fr.rt0, fr.rt1, fr.st);
+        ctx->launches++;
+        timer_mark(p, "Ray Trace", fr.st);
+        // the history = last frame's images of whichever rank owns the reprojected row (peer history, shard.cu): wait until every
+        // peer has finished writing them (tick epoch - 1), overlapped with the ray trace above
+        if (denoise && !fr.no_history && (rc = hr_peer_wait(p, 0, fr.epoch - 1, fr.st)) != HR_OK) return rc;
+    }
+    if (spp > 1) fr.final = { p->count, p->W, p->H, HR_FMT_R8_UINT };
+    else fr.final = { mask, (p->W + 7) / 8, (p->H + 3) / 4, HR_FMT_R32_UINT };
+    p->out_view[HR_SHADOWS_OUT_RAY_TRACE] = fr.final;
+    *mask_out   = mask;
+    *shared_out = shared;
+    return HR_OK;
+}
+
+// upsample (ray_traced_shadows.cpp:1219-1255, ray_traced_ao.cpp:918-957): the pass's last image to full resolution, the final output
+static void upsample_scalar(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const void* in, int in_channels, float sky_value, float power)
+{
+    hr_ctx* ctx = p->ctx;
+    launch_upsample_scalar(level_view(ctx, fr.pp, 0), cur, in, in_channels, sky_value, power, p->upsample_out, fr.up0, fr.up1, fr.st);
+    ctx->launches++;
+    timer_mark(p, "Upsample", fr.st);
+    fr.final = { p->upsample_out, p->W0, p->H0, HR_FMT_R16F };
+    p->out_view[HR_SHADOWS_OUT_UPSAMPLE] = fr.final;
 }
 
 static int check_render_ready(hr_pass* p, const hr_frame* f, const void* params, bool needs_scene)
@@ -808,32 +934,28 @@ void hr_shadows_default_params(hr_shadows_params* p)
 
 int hr_shadows_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** out)
 {
-    int rc = pass_common_create(ctx, width, height, scale, PASS_SHADOWS, out);
-    if (rc != HR_OK) return rc;
-    hr_pass*     p  = *out;
-    const size_t px = (size_t)p->W * p->H, mw = (p->W + 7) / 8, mh = (p->H + 3) / 4, tw = (p->W + 7) / 8, th = (p->H + 7) / 8;
-#define A(call) do { rc = (call); if (rc != HR_OK) { hr_pass_destroy(p); *out = nullptr; return rc; } } while (0)
-    A(pass_alloc(p, p->mask, mw * mh));
-    A(pass_alloc(p, p->temporal_out, px));
-    A(pass_alloc(p, p->moments[0], px));
-    A(pass_alloc(p, p->moments[1], px));
-    A(pass_alloc(p, p->prev_image[0], px));
-    A(pass_alloc(p, p->prev_image[1], px));
-    A(pass_alloc(p, p->atrous[0], px));
-    A(pass_alloc(p, p->atrous[1], px));
-    A(pass_alloc(p, p->tile_flags, tw * th));
-    if (scale != HR_SCALE_FULL) A(pass_alloc(p, p->upsample_out, (size_t)p->W0 * p->H0));
-#undef A
-    rc = pass_alloc_rt_share(p);
-    if (rc != HR_OK) { hr_pass_destroy(p); *out = nullptr; return rc; }
-    void* hist[7] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
-    hr_peer_register(p, hist, 7);
-    for (int i = 0; i < 2; i++)
-    {
-        p->hist_view[HR_SHADOWS_OUT_PREV_IMAGE][i] = { p->prev_image[i], p->W, p->H, HR_FMT_RG16F };
-        p->hist_view[HR_SHADOWS_OUT_MOMENTS][i]    = { p->moments[i], p->W, p->H, HR_FMT_RGBA16F };
-    }
-    return HR_OK;
+    return pass_create(ctx, width, height, scale, PASS_SHADOWS, out, [](PassAllocs& A) {
+        hr_pass*     p  = A.p;
+        const size_t px = (size_t)p->W * p->H, mw = (p->W + 7) / 8, mh = (p->H + 3) / 4, tw = (p->W + 7) / 8, th = (p->H + 7) / 8;
+        A(p->mask, mw * mh);
+        A(p->temporal_out, px);
+        A(p->moments[0], px);
+        A(p->moments[1], px);
+        A(p->prev_image[0], px);
+        A(p->prev_image[1], px);
+        A(p->atrous[0], px);
+        A(p->atrous[1], px);
+        A(p->tile_flags, tw * th);
+        if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
+        pass_alloc_rt_share(A);
+        void* hist[7] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
+        hr_peer_register(p, hist, 7);
+        for (int i = 0; i < 2; i++)
+        {
+            p->hist_view[HR_SHADOWS_OUT_PREV_IMAGE][i] = { p->prev_image[i], p->W, p->H, HR_FMT_RG16F };
+            p->hist_view[HR_SHADOWS_OUT_MOMENTS][i]    = { p->moments[i], p->W, p->H, HR_FMT_RGBA16F };
+        }
+    });
 }
 
 int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* prm, void* stream)
@@ -849,27 +971,10 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
     const FrameConsts  fc  = make_consts(f, p);
     const GBufLevelDev cur = level_view(ctx, pp, p->scale), prev = level_view(ctx, !pp, p->scale);
     const size_t       px = (size_t)p->W * p->H;
-    // row-band sharding (shard.cu): owned band [b0,b1); temporal / a-trous on band +- the rows the a-trous chain erodes (16 for
-    // the default 4 iterations at radius 1: 1+2+4+8 = 15), ray trace 8 rows further (17x17 mean of the temporal stage).
     const int spp = prm->spp > 1 ? prm->spp : 1;
     HR_REQUIRE(ctx, spp <= 255, HR_ERR_UNSUPPORTED, "hr_shadows_render: spp must be <= 255");
-    const int halo = ctx->world > 1 && prm->denoise ? atrous_halo_rows(prm->radius, prm->filter_iterations) : 0;
-    int b0, b1, rt0, rt1, row0, row1;
-    hr_band(ctx, p->H, &b0, &b1);
-    hr_extend(b0, b1, ctx->world > 1 && prm->denoise ? halo + 8 : 0, p->H, &rt0, &rt1);
-    hr_extend(b0, b1, halo, p->H, &row0, &row1);
-    p->last_rows[0] = row0; p->last_rows[1] = row1;
-    timer_begin(p, st);
-
-    if (ctx->world > 1 && ctx->nccl_comm && !p->peers_linked)
-    { // first sharded render: map the peers' history images (collective, shard.cu)
-        rc = hr_peer_link_ipc(p, st);
-        if (rc != HR_OK) return rc;
-    }
-    const int  epoch      = ++p->epoch;
-    p->n_renders++;
-    const bool no_history = p->first;
-    bool       signalled  = false;
+    PassFrame fr;
+    if ((rc = frame_begin(p, f, prm->denoise, halo_plan(PASS_SHADOWS, prm->radius, prm->filter_iterations, 0), st, &fr)) != HR_OK) return rc;
     hr_wait_exchange(p, st); // last frame's gather of the final output (side stream) reads images this frame rewrites
     // clear_images (ray_traced_shadows.cpp:938-968): first frame => history image and moments[!pp] = 0.  The reprojection
     // kernel is told not to read any history on that frame (same values as reading the cleared images, and no peer can be
@@ -878,58 +983,21 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
     {
         HR_CUDA(ctx, cudaMemsetAsync(p->prev_image[!pp], 0, px * sizeof(__half2), st));
         HR_CUDA(ctx, cudaMemsetAsync(p->moments[!pp], 0, px * sizeof(uint2), st));
-        p->first = false;
+        p->first = false; // nothing below reads it (unlike reflections)
     }
-    // ray_trace (:972-1011).  Linked to peers: this rank traces its cost-balanced share of the WHOLE image and stores the
-    // mask words into every rank's mask image (no halo re-trace); otherwise its band +- (denoise halo + 8) rows into its own image.
-    RtShare    rts;
-    const bool shared_rt = spp == 1 && hr_rt_share(p, epoch & 1, &rts);
-    uint32_t*  mask      = shared_rt ? p->mask_pp[epoch & 1] : p->mask;
-    if (shared_rt)
-    {
-        launch_shadows_ray_trace_shared(cur, hr_bvh_view(ctx->scene), fc, prm->bias, ctx->d_sobol, ctx->d_scr_rank, rts, st);
-        ctx->launches++;
-        rc = hr_rt_share_finish(p, epoch & 1, epoch, st);
-        if (rc != HR_OK) return rc;
-        timer_mark(p, "Ray Trace", st);
-        // every rank's share of this frame's mask (and cost table) has arrived, and last frame's history is complete
-        rc = hr_rt_wait_partition(p, epoch & 1, epoch, (prm->denoise && !no_history) ? epoch - 1 : 0, st);
-        if (rc != HR_OK) return rc;
-        timer_mark(p, "Mask Exchange Wait", st);
-    }
-    else if (spp > 1)
-    { // SURVEY.md §8d: spp rays per pixel into an 8-bit count image (allocated on first use)
-        if (!p->count) { rc = pass_alloc(p, p->count, px); if (rc != HR_OK) return rc; }
-        launch_shadows_ray_trace_count(cur, hr_bvh_view(ctx->scene), fc, prm->bias, ctx->d_sobol, bn_table(ctx, spp), p->count, spp, rt0, rt1, st);
-        ctx->launches++;
-        timer_mark(p, "Ray Trace", st);
-    }
-    else
-    {
-        launch_shadows_ray_trace(cur, hr_bvh_view(ctx->scene), fc, prm->bias, ctx->d_sobol, ctx->d_scr_rank, mask, rt0, rt1, st);
-        ctx->launches++;
-        timer_mark(p, "Ray Trace", st);
-    }
-    if (spp > 1) set_view(p, HR_SHADOWS_OUT_RAY_TRACE, p->count, p->W, p->H, HR_FMT_R8_UINT);
-    else set_view(p, HR_SHADOWS_OUT_RAY_TRACE, mask, (p->W + 7) / 8, (p->H + 3) / 4, HR_FMT_R32_UINT);
-    void* final_ptr = spp > 1 ? (void*)p->count : (void*)mask;
-    int   final_w = spp > 1 ? p->W : (p->W + 7) / 8, final_h = spp > 1 ? p->H : (p->H + 3) / 4, final_fmt = spp > 1 ? HR_FMT_R8_UINT : HR_FMT_R32_UINT;
+    uint32_t* mask;
+    bool      shared_rt;
+    if ((rc = trace_mask(p, fr, cur, fc, prm->bias, 0.0f, spp, prm->denoise != 0, &mask, &shared_rt)) != HR_OK) return rc;
     if (prm->denoise)
     {
         // temporal_accumulation (:1041-1090); reset_args (:1015-1037) is subsumed by the per-tile flag image.
-        // History = prev_image[!pp] / moments[!pp] of whichever rank owns the reprojected row (peer history, shard.cu):
-        // wait until every peer has finished writing them (tick epoch-1), overlapped with the ray trace above.
+        // History = prev_image[!pp] / moments[!pp] of whichever rank owns the reprojected row (peer history, shard.cu).
         HistPeers hist;
-        hr_peer_hist(p, !pp, 2 + !pp, p->H, no_history, &hist);
-        if (!no_history && !shared_rt)
-        {
-            rc = hr_peer_wait(p, 0, epoch - 1, st);
-            if (rc != HR_OK) return rc;
-        }
+        hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
         if (spp > 1)
-            launch_shadows_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, row0, row1, st);
+            launch_shadows_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
         else
-            launch_shadows_temporal(cur, prev, mask, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, row0, row1, st);
+            launch_shadows_temporal(cur, prev, mask, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;
         timer_mark(p, "Temporal Accumulation", st);
         // a_trous_filter (:1094-1215).  The reference ping-pongs image[0]/image[1] and copies the output of
@@ -948,22 +1016,19 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
                 dst = p->atrous[toggle];
             }
             const float power = (i == prm->filter_iterations - 1) ? prm->power : 0.0f;
-            launch_shadows_atrous(cur, in, p->tile_flags, prm->radius, 1 << i, prm->phi_visibility, prm->phi_normal, prm->sigma_depth, power, dst, row0, row1, st);
+            launch_shadows_atrous(cur, in, p->tile_flags, prm->radius, 1 << i, prm->phi_visibility, prm->phi_normal, prm->sigma_depth, power, dst, fr.row0, fr.row1, st);
             ctx->launches++;
             if (i == prm->feedback_iteration)
             {
                 if (dst != hist_out) HR_CUDA(ctx, cudaMemcpyAsync(hist_out, dst, px * sizeof(__half2), cudaMemcpyDeviceToDevice, st));
                 fed_back = true;
-                // both history images of this frame (moments[pp] from the temporal stage, prev_image[pp]) are complete
-                rc = hr_peer_signal(p, 0, epoch, st);
-                if (rc != HR_OK) return rc;
-                signalled = true;
+                // shadows signal here, not after the temporal stage: prev_image[pp] is only complete after the feedback iteration
+                if ((rc = frame_signal(p, fr)) != HR_OK) return rc;
             }
             in     = dst;
             last   = dst;
             toggle = !toggle;
-            static const char* names[8] = { "A-Trous 0", "A-Trous 1", "A-Trous 2", "A-Trous 3", "A-Trous 4", "A-Trous 5", "A-Trous 6", "A-Trous 7" };
-            timer_mark(p, names[i], st);
+            timer_mark(p, atrous_stage_names[i], st);
         }
         if (!fed_back)
         { // no feedback: the history image keeps its previous contents, like the reference's single prev_image
@@ -974,32 +1039,18 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
         set_view(p, HR_SHADOWS_OUT_MOMENTS, p->moments[pp], p->W, p->H, HR_FMT_RGBA16F);
         set_view(p, HR_SHADOWS_OUT_PREV_IMAGE, hist_out, p->W, p->H, HR_FMT_RG16F);
         set_view(p, HR_SHADOWS_OUT_TILE_FLAGS, p->tile_flags, (p->W + 7) / 8, (p->H + 7) / 8, HR_FMT_R8_UINT);
-        final_ptr = last; final_w = p->W; final_h = p->H; final_fmt = HR_FMT_RG16F;
-        if (p->scale != HR_SCALE_FULL)
-        { // upsample (:1219-1255)
-            const GBufLevelDev g0 = level_view(ctx, pp, 0);
-            launch_upsample_scalar(g0, cur, last, 2, 0.0f, 0.0f, p->upsample_out, b0 << p->scale, b1 >= p->H ? p->H0 : (b1 << p->scale), st);
-            ctx->launches++;
-            timer_mark(p, "Upsample", st);
-            set_view(p, HR_SHADOWS_OUT_UPSAMPLE, p->upsample_out, p->W0, p->H0, HR_FMT_R16F);
-            final_ptr = p->upsample_out; final_w = p->W0; final_h = p->H0; final_fmt = HR_FMT_R16F;
-        }
+        fr.final = { last, p->W, p->H, HR_FMT_RG16F };
+        if (p->scale != HR_SCALE_FULL) upsample_scalar(p, fr, cur, last, 2, 0.0f, 0.0f);
     }
-    if (!signalled)
-    {
-        rc = hr_peer_signal(p, 0, epoch, st);
-        if (rc != HR_OK) return rc;
-    }
-    set_view(p, 100, final_ptr, final_w, final_h, final_fmt);
-    HR_CHECK_LAUNCH(ctx);
+    if ((rc = frame_end(p, fr)) != HR_OK) return rc;
     if (ctx->world > 1 && ctx->gather_final && !(shared_rt && !prm->denoise))
     { // every rank ends up with the complete final output (the history stays distributed: peer history, shard.cu)
         ExchangeItem it[2];
         int          n = 0;
         if (prm->denoise)
         {
-            if (final_fmt == HR_FMT_RG16F) it[n++] = { final_ptr, (size_t)p->W * 4, p->H, 0, 1, p->H };
-            if (final_fmt == HR_FMT_R16F) it[n++] = { final_ptr, (size_t)p->W0 * 2, p->H, p->scale, 1, p->H0 };
+            if (fr.final.fmt == HR_FMT_RG16F) it[n++] = { fr.final.p, (size_t)p->W * 4, p->H, 0, 1, p->H };
+            if (fr.final.fmt == HR_FMT_R16F) it[n++] = { fr.final.p, (size_t)p->W0 * 2, p->H, p->scale, 1, p->H0 };
         }
         else it[n++] = { mask, (size_t)((p->W + 7) / 8) * 4, p->H, 0, 4, (p->H + 3) / 4 };
         rc = hr_shard_exchange(p, it, n, st);
@@ -1019,31 +1070,27 @@ void hr_ao_default_params(hr_ao_params* p)
 
 int hr_ao_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** out)
 {
-    int rc = pass_common_create(ctx, width, height, scale, PASS_AO, out);
-    if (rc != HR_OK) return rc;
-    hr_pass*     p  = *out;
-    const size_t px = (size_t)p->W * p->H, mw = (p->W + 7) / 8, mh = (p->H + 3) / 4, tw = (p->W + 7) / 8, th = (p->H + 7) / 8;
-#define A(call) do { rc = (call); if (rc != HR_OK) { hr_pass_destroy(p); *out = nullptr; return rc; } } while (0)
-    A(pass_alloc(p, p->mask, mw * mh));
-    for (int i = 0; i < 2; i++)
-    {
-        A(pass_alloc(p, p->ao_color[i], px));
-        A(pass_alloc(p, p->ao_len[i], px));
-        A(pass_alloc(p, p->ao_blur[i], px));
-    }
-    A(pass_alloc(p, p->tile_flags, tw * th));
-    if (scale != HR_SCALE_FULL) A(pass_alloc(p, p->upsample_out, (size_t)p->W0 * p->H0));
-#undef A
-    rc = pass_alloc_rt_share(p);
-    if (rc != HR_OK) { hr_pass_destroy(p); *out = nullptr; return rc; }
-    void* hist[7] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
-    hr_peer_register(p, hist, 7);
-    for (int i = 0; i < 2; i++)
-    {
-        p->hist_view[HR_AO_OUT_TEMPORAL_ACCUMULATION][i] = { p->ao_color[i], p->W, p->H, HR_FMT_R16F };
-        p->hist_view[HR_AO_OUT_HISTORY_LENGTH][i]        = { p->ao_len[i], p->W, p->H, HR_FMT_R16F };
-    }
-    return HR_OK;
+    return pass_create(ctx, width, height, scale, PASS_AO, out, [](PassAllocs& A) {
+        hr_pass*     p  = A.p;
+        const size_t px = (size_t)p->W * p->H, mw = (p->W + 7) / 8, mh = (p->H + 3) / 4, tw = (p->W + 7) / 8, th = (p->H + 7) / 8;
+        A(p->mask, mw * mh);
+        for (int i = 0; i < 2; i++)
+        {
+            A(p->ao_color[i], px);
+            A(p->ao_len[i], px);
+            A(p->ao_blur[i], px);
+        }
+        A(p->tile_flags, tw * th);
+        if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
+        pass_alloc_rt_share(A);
+        void* hist[7] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
+        hr_peer_register(p, hist, 7);
+        for (int i = 0; i < 2; i++)
+        {
+            p->hist_view[HR_AO_OUT_TEMPORAL_ACCUMULATION][i] = { p->ao_color[i], p->W, p->H, HR_FMT_R16F };
+            p->hist_view[HR_AO_OUT_HISTORY_LENGTH][i]        = { p->ao_len[i], p->W, p->H, HR_FMT_R16F };
+        }
+    });
 }
 
 int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* stream)
@@ -1058,27 +1105,10 @@ int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* s
     const FrameConsts  fc  = make_consts(f, p);
     const GBufLevelDev cur = level_view(ctx, pp, p->scale), prev = level_view(ctx, !pp, p->scale);
     const size_t       px = (size_t)p->W * p->H;
-    // row-band sharding: the vertical blur runs on band +- 8 (the upsample reads one coarse row beyond the band) and reads
-    // +- blur_radius rows of the horizontal pass, which is pointwise in y over the temporal output; the temporal stage's
-    // 17x17 mean reads the ray mask 8 rows further
     const int spp = prm->spp > 1 ? prm->spp : 1;
     HR_REQUIRE(ctx, spp <= 255, HR_ERR_UNSUPPORTED, "hr_ao_render: spp must be <= 255");
-    const int halo = ctx->world > 1 && prm->denoise ? 8 + round_up8(prm->blur_radius) : 0;
-    int b0, b1, rt0, rt1, row0, row1, v0, v1;
-    hr_band(ctx, p->H, &b0, &b1);
-    hr_extend(b0, b1, ctx->world > 1 && prm->denoise ? halo + 8 : 0, p->H, &rt0, &rt1);
-    hr_extend(b0, b1, halo, p->H, &row0, &row1);
-    hr_extend(b0, b1, ctx->world > 1 && prm->denoise ? 8 : 0, p->H, &v0, &v1);
-    p->last_rows[0] = row0; p->last_rows[1] = row1;
-    timer_begin(p, st);
-    if (ctx->world > 1 && ctx->nccl_comm && !p->peers_linked)
-    {
-        rc = hr_peer_link_ipc(p, st);
-        if (rc != HR_OK) return rc;
-    }
-    const int  epoch      = ++p->epoch;
-    p->n_renders++;
-    const bool no_history = p->first;
+    PassFrame fr;
+    if ((rc = frame_begin(p, f, prm->denoise, halo_plan(PASS_AO, 0, 0, prm->blur_radius), st, &fr)) != HR_OK) return rc;
     hr_wait_exchange(p, st);
     if (p->first)
     { // clear_images, ray_traced_ao.cpp:829-860 (see hr_shadows_render for the first-frame / peer rules)
@@ -1086,82 +1116,32 @@ int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* s
         HR_CUDA(ctx, cudaMemsetAsync(p->ao_color[!pp], 0, px * sizeof(__half), st));
         p->first = false;
     }
-    RtShare    rts;
-    const bool shared_rt = spp == 1 && hr_rt_share(p, epoch & 1, &rts); // see hr_shadows_render
-    uint32_t*  mask      = shared_rt ? p->mask_pp[epoch & 1] : p->mask;
-    if (shared_rt)
-    {
-        launch_ao_ray_trace_shared(cur, hr_bvh_view(ctx->scene), fc, prm->ray_length, prm->bias, ctx->d_sobol, ctx->d_scr_rank, rts, st);
-        ctx->launches++;
-        rc = hr_rt_share_finish(p, epoch & 1, epoch, st);
-        if (rc != HR_OK) return rc;
-        timer_mark(p, "Ray Trace", st);
-        rc = hr_rt_wait_partition(p, epoch & 1, epoch, (prm->denoise && !no_history) ? epoch - 1 : 0, st);
-        if (rc != HR_OK) return rc;
-        timer_mark(p, "Mask Exchange Wait", st);
-    }
-    else if (spp > 1)
-    {
-        if (!p->count) { rc = pass_alloc(p, p->count, px); if (rc != HR_OK) return rc; }
-        launch_ao_ray_trace_count(cur, hr_bvh_view(ctx->scene), fc, prm->ray_length, prm->bias, ctx->d_sobol, bn_table(ctx, spp), p->count, spp, rt0, rt1, st);
-        ctx->launches++;
-        timer_mark(p, "Ray Trace", st);
-    }
-    else
-    {
-        launch_ao_ray_trace(cur, hr_bvh_view(ctx->scene), fc, prm->ray_length, prm->bias, ctx->d_sobol, ctx->d_scr_rank, mask, rt0, rt1, st);
-        ctx->launches++;
-        timer_mark(p, "Ray Trace", st);
-    }
-    if (spp > 1) set_view(p, HR_AO_OUT_RAY_TRACE, p->count, p->W, p->H, HR_FMT_R8_UINT);
-    else set_view(p, HR_AO_OUT_RAY_TRACE, mask, (p->W + 7) / 8, (p->H + 3) / 4, HR_FMT_R32_UINT);
-    void* final_ptr = spp > 1 ? (void*)p->count : (void*)mask;
-    int   final_w = spp > 1 ? p->W : (p->W + 7) / 8, final_h = spp > 1 ? p->H : (p->H + 3) / 4, final_fmt = spp > 1 ? HR_FMT_R8_UINT : HR_FMT_R32_UINT;
-    bool  signalled = false;
+    uint32_t* mask;
+    bool      shared_rt;
+    if ((rc = trace_mask(p, fr, cur, fc, prm->ray_length, prm->bias, spp, prm->denoise != 0, &mask, &shared_rt)) != HR_OK) return rc;
     if (prm->denoise)
     {
         // history = ao_color[!pp] / ao_len[!pp] of the rank that owns the reprojected row (peer history, shard.cu)
         HistPeers hist;
-        hr_peer_hist(p, !pp, 2 + !pp, p->H, no_history, &hist);
-        if (!no_history && !shared_rt)
-        {
-            rc = hr_peer_wait(p, 0, epoch - 1, st);
-            if (rc != HR_OK) return rc;
-        }
-        if (spp > 1) launch_ao_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, row0, row1, st);
-        else launch_ao_temporal(cur, prev, mask, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, row0, row1, st);
+        hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
+        if (spp > 1) launch_ao_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
+        else launch_ao_temporal(cur, prev, mask, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;
-        rc = hr_peer_signal(p, 0, epoch, st); // this frame's history (ao_color[pp], ao_len[pp]) is complete
-        if (rc != HR_OK) return rc;
-        signalled = true;
+        if ((rc = frame_signal(p, fr)) != HR_OK) return rc; // this frame's history (ao_color[pp], ao_len[pp]) is complete
         timer_mark(p, "Temporal Accumulation", st);
         // bilateral_blur (:1032-1137): pass labelled "Vertical" uses direction (1,0), then (0,1)
-        launch_ao_blur(cur, p->ao_color[pp], p->tile_flags, f->z_buffer_params, 1, 0, prm->blur_radius, p->ao_blur[0], row0, row1, st);
-        launch_ao_blur(cur, p->ao_blur[0], p->tile_flags, f->z_buffer_params, 0, 1, prm->blur_radius, p->ao_blur[1], v0, v1, st);
+        launch_ao_blur(cur, p->ao_color[pp], p->tile_flags, f->z_buffer_params, 1, 0, prm->blur_radius, p->ao_blur[0], fr.row0, fr.row1, st);
+        launch_ao_blur(cur, p->ao_blur[0], p->tile_flags, f->z_buffer_params, 0, 1, prm->blur_radius, p->ao_blur[1], fr.v0, fr.v1, st);
         ctx->launches += 2;
         timer_mark(p, "Bilateral Blur", st);
         set_view(p, HR_AO_OUT_TEMPORAL_ACCUMULATION, p->ao_color[pp], p->W, p->H, HR_FMT_R16F);
         set_view(p, HR_AO_OUT_HISTORY_LENGTH, p->ao_len[pp], p->W, p->H, HR_FMT_R16F);
         set_view(p, HR_AO_OUT_BILATERAL_BLUR, p->ao_blur[1], p->W, p->H, HR_FMT_R16F);
         set_view(p, HR_AO_OUT_TILE_FLAGS, p->tile_flags, (p->W + 7) / 8, (p->H + 7) / 8, HR_FMT_R8_UINT);
-        final_ptr = p->ao_blur[1]; final_w = p->W; final_h = p->H; final_fmt = HR_FMT_R16F;
-        if (p->scale != HR_SCALE_FULL)
-        { // upsample (:918-957)
-            const GBufLevelDev g0 = level_view(ctx, pp, 0);
-            launch_upsample_scalar(g0, cur, p->ao_blur[1], 1, 1.0f, prm->power, p->upsample_out, b0 << p->scale, b1 >= p->H ? p->H0 : (b1 << p->scale), st);
-            ctx->launches++;
-            timer_mark(p, "Upsample", st);
-            set_view(p, HR_AO_OUT_UPSAMPLE, p->upsample_out, p->W0, p->H0, HR_FMT_R16F);
-            final_ptr = p->upsample_out; final_w = p->W0; final_h = p->H0; final_fmt = HR_FMT_R16F;
-        }
+        fr.final = { p->ao_blur[1], p->W, p->H, HR_FMT_R16F };
+        if (p->scale != HR_SCALE_FULL) upsample_scalar(p, fr, cur, p->ao_blur[1], 1, 1.0f, prm->power);
     }
-    if (!signalled)
-    {
-        rc = hr_peer_signal(p, 0, epoch, st);
-        if (rc != HR_OK) return rc;
-    }
-    set_view(p, 100, final_ptr, final_w, final_h, final_fmt);
-    HR_CHECK_LAUNCH(ctx);
+    if ((rc = frame_end(p, fr)) != HR_OK) return rc;
     if (ctx->world > 1 && ctx->gather_final && !(shared_rt && !prm->denoise))
     {
         ExchangeItem it[4];
@@ -1194,46 +1174,44 @@ int hr_pass_output(hr_pass* p, int which, hr_image* out)
     return HR_OK;
 }
 
-// hr_pass_download without the host synchronisation: the caller orders it with its own stream / event waits.
-int hr_pass_download_async(hr_pass* p, int which, void* dst, size_t bytes, void* stream)
-{
-    hr_image img;
-    int      rc = hr_pass_output(p, which, &img);
-    if (rc != HR_OK) return rc;
-    hr_ctx*      ctx  = p->ctx;
-    const size_t need = (size_t)img.width * img.height * texel_size(img.format);
-    HR_REQUIRE(ctx, dst && bytes == need, HR_ERR_INVALID_ARG, "hr_pass_download_async: byte count mismatch");
-    hr_wait_exchange(p, (cudaStream_t)stream);
-    HR_CUDA(ctx, cudaMemcpyAsync(dst, img.data, need, cudaMemcpyDefault, (cudaStream_t)stream));
-    return HR_OK;
-}
+} // extern "C"
 
-// Rows [row0,row1) of an image (a rank's own band of a distributed output), asynchronous like hr_pass_download_async.
-int hr_pass_download_rows_async(hr_pass* p, int which, int row0, int row1, void* dst, size_t bytes, void* stream)
+// Rows [row0,row1) of output `which` (all of them when all_rows) into dst, enqueued on `st` after the pass's pending exchange;
+// `who` names the entry point in error messages.
+static int download_rows(hr_pass* p, int which, bool all_rows, int row0, int row1, void* dst, size_t bytes, cudaMemcpyKind kind, cudaStream_t st, const char* who)
 {
     hr_image img;
     int      rc = hr_pass_output(p, which, &img);
     if (rc != HR_OK) return rc;
     hr_ctx* ctx = p->ctx;
-    HR_REQUIRE(ctx, row0 >= 0 && row1 >= row0 && row1 <= img.height, HR_ERR_INVALID_ARG, "hr_pass_download_rows_async: bad row range");
+    if (all_rows) { row0 = 0; row1 = img.height; }
+    if (!(row0 >= 0 && row1 >= row0 && row1 <= img.height)) { hr_set_error(ctx, "%s: bad row range", who); return HR_ERR_INVALID_ARG; }
     const size_t row_bytes = (size_t)img.width * texel_size(img.format), need = row_bytes * (size_t)(row1 - row0);
-    HR_REQUIRE(ctx, dst && bytes == need, HR_ERR_INVALID_ARG, "hr_pass_download_rows_async: byte count mismatch");
-    hr_wait_exchange(p, (cudaStream_t)stream);
-    if (need) HR_CUDA(ctx, cudaMemcpyAsync(dst, static_cast<const char*>(img.data) + row_bytes * row0, need, cudaMemcpyDefault, (cudaStream_t)stream));
+    if (!(dst && bytes == need)) { hr_set_error(ctx, "%s: byte count mismatch", who); return HR_ERR_INVALID_ARG; }
+    hr_wait_exchange(p, st);
+    if (need) HR_CUDA(ctx, cudaMemcpyAsync(dst, static_cast<const char*>(img.data) + row_bytes * row0, need, kind, st));
     return HR_OK;
+}
+
+extern "C" {
+
+// hr_pass_download without the host synchronisation: the caller orders it with its own stream / event waits.
+int hr_pass_download_async(hr_pass* p, int which, void* dst, size_t bytes, void* stream)
+{
+    return download_rows(p, which, true, 0, 0, dst, bytes, cudaMemcpyDefault, (cudaStream_t)stream, "hr_pass_download_async");
+}
+
+// Rows [row0,row1) of an image (a rank's own band of a distributed output), asynchronous like hr_pass_download_async.
+int hr_pass_download_rows_async(hr_pass* p, int which, int row0, int row1, void* dst, size_t bytes, void* stream)
+{
+    return download_rows(p, which, false, row0, row1, dst, bytes, cudaMemcpyDefault, (cudaStream_t)stream, "hr_pass_download_rows_async");
 }
 
 int hr_pass_download(hr_pass* p, int which, void* dst, size_t bytes, void* stream)
 {
-    hr_image img;
-    int      rc = hr_pass_output(p, which, &img);
+    const int rc = download_rows(p, which, true, 0, 0, dst, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream, "hr_pass_download");
     if (rc != HR_OK) return rc;
-    hr_ctx*      ctx  = p->ctx;
-    const size_t need = (size_t)img.width * img.height * texel_size(img.format);
-    HR_REQUIRE(ctx, dst && bytes == need, HR_ERR_INVALID_ARG, "hr_pass_download: byte count mismatch");
-    hr_wait_exchange(p, (cudaStream_t)stream);
-    HR_CUDA(ctx, cudaMemcpyAsync(dst, img.data, need, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-    HR_CUDA(ctx, cudaStreamSynchronize((cudaStream_t)stream));
+    HR_CUDA(p->ctx, cudaStreamSynchronize((cudaStream_t)stream));
     return HR_OK;
 }
 

@@ -291,10 +291,6 @@ inline int hr_rt_share_cap(int MH, int world) { const int c = 2 * ((MH + world -
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out); // false when the pass is not linked to peers
 int  hr_rt_share_finish(hr_pass* p, int parity, int tick, cudaStream_t st); // push costs, signal the ray-trace tick
 int  hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cudaStream_t st); // wait for the peers' ticks, then next frame's bounds
-void launch_shadows_ray_trace_shared(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                                     const RtShare& sh, cudaStream_t st);
-void launch_ao_ray_trace_shared(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                                const uint8_t* sr, const RtShare& sh, cudaStream_t st);
 // Interleaved cooperative ray trace of the reflections pass (shard.cu): rank r traces the 8-row chunks c with c % world == r of the
 // WHOLE image into its own image and copies every chunk to the ranks whose denoise stages read it (rows [need0[q], need1[q]));
 // the last block publishes the ray-trace tick.
@@ -352,18 +348,18 @@ inline bool hr_once_per_device(bool (&done)[64])
 }
 
 
-void launch_shadows_ray_trace(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                              uint32_t* mask, int row0, int row1, cudaStream_t st);
-void launch_ao_ray_trace(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                         const uint8_t* sr, uint32_t* mask, int row0, int row1, cudaStream_t st);
-void launch_shadows_ray_trace_count(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                                    uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
-void launch_ao_ray_trace_count(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                               const uint8_t* sr, uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
 void launch_shadows_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
                                    float alpha, float moments_alpha, __half2* out, uint2* moments_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 void launch_ao_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
                               float alpha, __half* out, __half* len_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
+// trace.cu: the shadows (kind PASS_SHADOWS, K1: p0 = bias) and AO (PASS_AO, K7: p0 = ray length, p1 = bias) ray traces into the mask image,
+// the mask images of the cooperative trace (shard.cu) or, spp > 1, the count image
+void launch_ray_trace_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
+                           uint32_t* mask, int row0, int row1, cudaStream_t st);
+void launch_ray_trace_mask_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
+                                  const uint8_t* sr, const RtShare& sh, cudaStream_t st);
+void launch_ray_trace_count(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
+                            uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
 void launch_trace_any(const BvhDev& bvh, const float* rays, size_t n, uint32_t* out, cudaStream_t st);
 void launch_trace_closest(const BvhDev& bvh, const float* rays, size_t n, float* out_t, uint32_t* out_prim, float* out_uv, cudaStream_t st);
 

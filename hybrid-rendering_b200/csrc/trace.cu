@@ -208,55 +208,32 @@ __global__ void k_trace_closest(BvhDev bvh, const float* __restrict__ rays, size
 
 static inline dim3 mask_grid(int W, int mrow0, int mrow1) { return dim3(((W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, mrow1 - mrow0, 1); }
 
-void launch_shadows_ray_trace(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                              uint32_t* mask, int row0, int row1, cudaStream_t st)
+// kind: PASS_SHADOWS (K1, p0 = bias) or PASS_AO (K7, p0 = ray length, p1 = bias)
+void launch_ray_trace_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
+                           uint32_t* mask, int row0, int row1, cudaStream_t st)
 {
     const int mrow0 = row0 / 4, mrow1 = (row1 + 3) / 4;
     if (mrow1 <= mrow0) return;
-    k_ray_trace_mask<0><<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, bias, 0.0f, sobol, sr, mask, mrow0, mrow1);
-}
-
-void launch_ao_ray_trace(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                         const uint8_t* sr, uint32_t* mask, int row0, int row1, cudaStream_t st)
-{
-    const int mrow0 = row0 / 4, mrow1 = (row1 + 3) / 4;
-    if (mrow1 <= mrow0) return;
-    k_ray_trace_mask<1><<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, ray_length, bias, sobol, sr, mask, mrow0, mrow1);
+    const auto k = kind == PASS_AO ? k_ray_trace_mask<1> : k_ray_trace_mask<0>;
+    k<<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, sobol, sr, mask, mrow0, mrow1);
 }
 
 // the grid covers the largest share hr_rt_wait_partition may hand to one rank
-static inline dim3 shared_grid(int W, int H, int world)
+void launch_ray_trace_mask_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
+                                  const uint8_t* sr, const RtShare& sh, cudaStream_t st)
 {
-    const int MH = (H + 3) / 4;
-    return dim3(((W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, hr_rt_share_cap(MH, world), 1);
+    const dim3 grid(((g.W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, hr_rt_share_cap((g.H + 3) / 4, sh.world), 1);
+    const auto k = kind == PASS_AO ? k_ray_trace_mask_shared<1> : k_ray_trace_mask_shared<0>;
+    k<<<grid, RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, sobol, sr, sh);
 }
 
-void launch_shadows_ray_trace_shared(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                                     const RtShare& sh, cudaStream_t st)
-{
-    k_ray_trace_mask_shared<0><<<shared_grid(g.W, g.H, sh.world), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, bias, 0.0f, sobol, sr, sh);
-}
-
-void launch_ao_ray_trace_shared(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                                const uint8_t* sr, const RtShare& sh, cudaStream_t st)
-{
-    k_ray_trace_mask_shared<1><<<shared_grid(g.W, g.H, sh.world), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, ray_length, bias, sobol, sr, sh);
-}
-
-void launch_shadows_ray_trace_count(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float bias, const uint8_t* sobol, const uint8_t* sr,
-                                    uint8_t* count, int spp, int row0, int row1, cudaStream_t st)
+void launch_ray_trace_count(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
+                            uint8_t* count, int spp, int row0, int row1, cudaStream_t st)
 {
     const int mrow0 = row0 / 4, mrow1 = (row1 + 3) / 4;
     if (mrow1 <= mrow0) return;
-    k_ray_trace_count<0><<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, bias, 0.0f, sobol, sr, count, spp, mrow0, mrow1);
-}
-
-void launch_ao_ray_trace_count(const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float ray_length, float bias, const uint8_t* sobol,
-                               const uint8_t* sr, uint8_t* count, int spp, int row0, int row1, cudaStream_t st)
-{
-    const int mrow0 = row0 / 4, mrow1 = (row1 + 3) / 4;
-    if (mrow1 <= mrow0) return;
-    k_ray_trace_count<1><<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, ray_length, bias, sobol, sr, count, spp, mrow0, mrow1);
+    const auto k = kind == PASS_AO ? k_ray_trace_count<1> : k_ray_trace_count<0>;
+    k<<<mask_grid(g.W, mrow0, mrow1), RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, sobol, sr, count, spp, mrow0, mrow1);
 }
 
 void launch_trace_any(const BvhDev& bvh, const float* rays, size_t n, uint32_t* out, cudaStream_t st)

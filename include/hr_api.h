@@ -535,7 +535,10 @@ HR_API int hr_pass_stage_times(hr_pass* pass, const char** names, float* ms, int
  * HR_ERR_INVALID_ARG and changes nothing.  None of them changes a result bit of the visibility masks; key 6 values 2 and 3 agree to
  * the last fp16 bit. */
 HR_API int hr_debug_set(int key, int value);
-/* Number of kernels this library launched since the context was created (bench.py gpu_launches). */
+/* Number of kernels this library launched since the context was created (bench.py gpu_launches).  Each kernel counts once.
+ * Earlier versions counted the reflections ray trace (K12) as two launches, a leftover of a removed two-kernel form, so config 3's
+ * gpu_launches was one per frame higher.  tests/test_gpu_launch_count.py checks the count against the kernels torch.profiler
+ * records for every pass. */
 HR_API uint64_t hr_ctx_launch_count(hr_ctx* ctx);
 
 /* Work actually done by a pass (bench.py: roofline on processed bytes, Mrays/s on counted rays; SURVEY.md §8d).

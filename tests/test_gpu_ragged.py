@@ -14,6 +14,7 @@ DDGI and reflections, same_halves and the tone-map rule (widened/test_gpu_taa_to
 it is meant to cover.  Run with -s to print the largest RMSE / max-abs error of every stage per case.
 """
 import re
+import time
 
 import numpy as np
 import pytest
@@ -459,14 +460,41 @@ def test_peer_history_reflections_ragged_half_res():
 
 
 # ---------------------------------------------------------------------------------------------- which kernel ran
-def _kernel_names(run):
-    """demangled names of the kernels launched while `run` executes (torch.profiler, CUDA activities)"""
+_profiler_gap_s = [0.05]
+
+
+def kernels_launched(run, attempts=6):
+    """demangled names of the kernels launched while `run` executes, in start order (torch.profiler, CUDA activities; memcpy and
+    memset are not kernels).  The profiler drops the device records it places before its window opens, and in a long process the
+    device time stamps can drift tens of milliseconds from the host clock that opens it; so a marker kernel is launched on each
+    side of `run`, a gap inside the window: a cycle that recorded both markers recorded every kernel between them.  A cycle that
+    did not is a profiler failure: the gap doubles (and stays doubled) and `run` is profiled again (it must be repeatable)."""
+    from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
+    marker = torch.zeros(1, device="cuda")
+    for _ in range(attempts):
         torch.cuda.synchronize()
-    return {e.name for e in prof.events()}
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            time.sleep(_profiler_gap_s[0])
+            marker.add_(1)
+            torch.cuda.synchronize()
+            run()
+            torch.cuda.synchronize()
+            marker.add_(1)
+            torch.cuda.synchronize()
+            time.sleep(_profiler_gap_s[0])
+        ev = sorted((e for e in prof.events() if e.device_type == DeviceType.CUDA and not e.name.startswith(("Memcpy", "Memset"))),
+                    key=lambda e: e.time_range.start)
+        names = [e.name for e in ev]
+        if len(names) >= 2 and names[0] == names[-1] and not re.search(r"\bk_\w+[<(]", names[0]):
+            return names[1:-1]
+        _profiler_gap_s[0] = min(2 * _profiler_gap_s[0], 2.0)
+    raise AssertionError(f"torch.profiler did not record a complete cycle in {attempts} attempts; last cycle: {names}")
+
+
+def _kernel_names(run):
+    """the set of kernels launched while `run` executes"""
+    return set(kernels_launched(run))
 
 
 def _launched(names, kernel):
