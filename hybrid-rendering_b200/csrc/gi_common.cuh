@@ -143,6 +143,11 @@ __device__ __forceinline__ float2 texture_coord_fast(float3 dir, int probe_index
     return make_float2((tlx + (o.x + 1.0f) * 0.5f * a.side) * a.inv_w, (tly + (o.y + 1.0f) * 0.5f * a.side) * a.inv_h);
 }
 
+// sqrt(x) as x * rsqrt(x).  The rsqrt argument is clamped to the finite range: at x = +inf (an atlas texel that saturated fp16,
+// DESIGN.md §6) the product is then inf, the reference's sqrt(inf), not inf * rsqrt(inf) = inf * 0 = NaN, which
+// sample_irradiance's NaN guard would turn into a finite 0.5.  Finite x are unchanged.
+__device__ __forceinline__ float sqrt_mul_rsqrt(float x) { return x * rsqrtf(fminf(fmaxf(x, 1e-30f), 3.402823466e38f)); }
+
 // sample_irradiance, gi_common.glsl:188-320 (LINEAR_BLENDING undefined => sqrt-space blend).  A tolerance-checked colour
 // stage: reciprocal square roots / approximate reciprocals replace the IEEE sqrt + divide sequences (the IEEE forms made
 // K21 instruction-bound), the per-atlas constants are hoisted, and the probe loop is unrolled UNR
@@ -199,7 +204,7 @@ __device__ inline float3 sample_irradiance(const hr_ddgi_uniforms& d, const Atla
         const float3 pi = sample_irr_atlas(at.irr, gi_.W, gi_.H, tc);
         if (weight < 0.2f) weight *= weight * weight * (1.0f / (0.2f * 0.2f));
         weight *= tri.x * tri.y * tri.z;
-        sum_irr = sum_irr + f3(pi.x * rsqrtf(fmaxf(pi.x, 1e-30f)), pi.y * rsqrtf(fmaxf(pi.y, 1e-30f)), pi.z * rsqrtf(fmaxf(pi.z, 1e-30f))) * weight;
+        sum_irr = sum_irr + f3(sqrt_mul_rsqrt(pi.x), sqrt_mul_rsqrt(pi.y), sqrt_mul_rsqrt(pi.z)) * weight;
         sum_w += weight;
     }
     const float inv_w = __fdividef(1.0f, sum_w);

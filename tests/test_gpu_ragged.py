@@ -40,13 +40,14 @@ SIZES = [(250, 141), (251, 144), (7, 3), (1, 1)]
 
 
 def frames(W, H, n, pan_from=3, vertical=0.0, cam=CAM_SHADOWS_TEST, light=None):
-    """static camera, then a lateral pan of 0.05 / frame; `vertical` adds a vertical pan so history taps cross the bottom edge"""
+    """static camera, then a lateral pan of 0.05 / frame; `vertical` adds a vertical pan so history taps cross the bottom edge.
+    light: a light descriptor (None: the synthetic default sun), or a callable frame index -> descriptor for a light that changes"""
     (px, py, pz), (tx, ty, tz) = cam
     f = None
     for i in range(n):
         dx = 0.0 if i < pan_from else 0.05 * (i - pan_from + 1)
         dy = 0.0 if i < pan_from else vertical * (i - pan_from + 1)
-        f = pyhr.make_frame((px + dx, py + dy, pz), (tx + dx, ty - dy, tz), W, H, prev=f, num_frames=i, light=light)
+        f = pyhr.make_frame((px + dx, py + dy, pz), (tx + dx, ty - dy, tz), W, H, prev=f, num_frames=i, light=light(i) if callable(light) else light)
         yield i, f
 
 
@@ -177,26 +178,28 @@ def test_ao_blur_radius(blur_radius):
 
 
 # ---------------------------------------------------------------------------------------------- DDGI + reflections
-def check_ddgi(i, dd, odd, w):
-    """every DDGI output against the oracle: uniforms bytes and ray directions / hit distances exact, images under `close`"""
+def check_ddgi(i, dd, odd, w, cmp=close):
+    """every DDGI output against the oracle: uniforms bytes and ray directions / hit distances exact, images under `cmp`"""
     assert bytes(dd.uniforms()) == bytes(odd.u), f"frame {i}: DDGIUniforms differ"
     dird_c = dd.download(1).view(np.uint16)
     assert np.array_equal(dird_c, odd.dirdepth.reshape(dird_c.shape)), f"frame {i}: probe ray direction / hit distance not exact"
-    close(f16(dd.download(0)), O.h2f(odd.radiance).reshape(-1, odd.u.rays_per_probe, 4), f"frame {i} ddgi radiance", 2e-3, 0.05)
-    close(f16(dd.download(2)), O.h2f(odd.cur_irr), f"frame {i} irradiance atlas")
-    close(f16(dd.download(3)), O.h2f(odd.cur_dep), f"frame {i} depth atlas", 2e-3, 0.05)
-    close(f16(dd.download(4)), O.h2f(odd.sample), f"frame {i} ddgi sample")
+    cmp(f16(dd.download(0)), O.h2f(odd.radiance).reshape(-1, odd.u.rays_per_probe, 4), f"frame {i} ddgi radiance", 2e-3, 0.05)
+    cmp(f16(dd.download(2)), O.h2f(odd.cur_irr), f"frame {i} irradiance atlas")
+    cmp(f16(dd.download(3)), O.h2f(odd.cur_dep), f"frame {i} depth atlas", 2e-3, 0.05)
+    cmp(f16(dd.download(4)), O.h2f(odd.sample), f"frame {i} ddgi sample")
     w.add("ddgi irradiance", f16(dd.download(2)), O.h2f(odd.cur_irr))
     w.add("ddgi sample", f16(dd.download(4)), O.h2f(odd.sample))
 
 
 def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0, cam=CAM_SHADOWS_TEST,
-                light=None, ddgi_params=None, lut=None, ddgi_hook=None):
+                light=None, ddgi_params=None, lut=None, ddgi_hook=None, frame_hook=None, cmp=close):
     """test_gpu_gi_refl.run at any size and scale (DDGI sampled at the reflections' scale), fed by the device G-buffer producer.
     ddgi_params: overrides of the DDGI parameter block; lut: a BRDF LUT set on the context and the oracle (the reflections' IBL
     specular term, as in test_deferred); ddgi_hook(i, f, rot, dd, odd, fresh) runs before frame i's DDGI render and returns the
-    DDGI oracle to go on with (fresh() makes a new one from dd.params: a re-initialised grid).  scene: a SynthScene kind, or an
-    object with SynthScene's interface"""
+    DDGI oracle to go on with (fresh() makes a new one from dd.params: a re-initialised grid); frame_hook(i, dd, odd, rf, orf) runs
+    after frame i's comparisons.  cmp: the comparison of the DDGI and reflections images (`close`, or a rule with its signature; a
+    rule that sets cmp.stopped ends the run after the comparison that set it).
+    scene: a SynthScene kind, or an object with SynthScene's interface"""
     sc = pyhr.SynthScene(scene, tris) if isinstance(scene, int) else scene
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
@@ -233,23 +236,29 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
                 odd = ddgi_hook(i, f, rot, dd, odd, fresh)
             dd.render(f, rot)
             odd.render(ss, cur_g, f, rot)
-            check_ddgi(i, dd, odd, w)
+            check_ddgi(i, dd, odd, w, cmp)
+            if getattr(cmp, "stopped", False):
+                break
         rf.render(f, dd)
         orf.render(ss, cur_g, prev_g, f, bn, odd)
         prev_g = cur_g
         rt_c, rt_o = f16(rf.download(0)), O.h2f(orf.rt)
         assert np.array_equal(rt_c[..., 3], rt_o[..., 3]), f"frame {i}: reflection ray length (hit / miss / t) not exact"
-        close(rt_c[..., :3], rt_o[..., :3], f"frame {i} reflections ray trace", 1e-3, 0.02)
+        cmp(rt_c[..., :3], rt_o[..., :3], f"frame {i} reflections ray trace", 1e-3, 0.02)
         w.add("rt", rt_c[..., :3], rt_o[..., :3])
         if not rf.params.denoise:
+            if frame_hook:
+                frame_hook(i, dd, odd, rf, orf)
             continue
         assert np.array_equal(rf.download(6), orf.tile_flags), f"frame {i}: reflections tile classification"
         mo_c, mo_o = f16(rf.download(4)), O.h2f(orf.cur_moments)
         assert np.array_equal(mo_c[..., 2], mo_o[..., 2]), f"frame {i}: reflections history length"
         for name, got, want in (("temporal", f16(rf.download(1)), O.h2f(orf.cur_temporal)), ("moments", mo_c, mo_o),
                                 ("a-trous", f16(rf.download(2)), O.h2f(orf.atrous_out)), ("final", f16(rf.download(100)), O.h2f(orf.final))):
-            close(got, want, f"frame {i} reflections {name}")
+            cmp(got, want, f"frame {i} reflections {name}")
             w.add(name, got, want)
+        if frame_hook:
+            frame_hook(i, dd, odd, rf, orf)
     w.report()
     rf.destroy()
     if dd:

@@ -9,6 +9,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import light_cases as LC
 import oracle as O
 import pyhr
 import pt_indirect as PI
@@ -56,8 +57,14 @@ def shadows():
     ctx.close()
 
 
+# the spot / overhead-sun / horizon-sun / coloured cases of light_cases.py after the two of the CPU tests
+LIGHT_CASES = ["spot_band", "sun_overhead", "sun_horizon", "colored"]
+LIGHTS = LIGHTS + [LC.BY_ID[c].kw for c in LIGHT_CASES]
+LIGHT_IDS = ["directional", "point"] + LIGHT_CASES
+
+
 @pytest.mark.parametrize("size", [(192, 112), (251, 141)], ids=["192x112", "251x141"])
-@pytest.mark.parametrize("light_kw", LIGHTS, ids=["directional", "point"])
+@pytest.mark.parametrize("light_kw", LIGHTS, ids=LIGHT_IDS)
 @pytest.mark.parametrize("B", [2, 4])
 def test_indirect_matches_the_oracle(shadows, size, light_kw, B):
     ctx, ss = shadows

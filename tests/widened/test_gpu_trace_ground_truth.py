@@ -5,6 +5,7 @@ silhouette is a full-scale difference in one pixel, so a handful of outliers are
 import numpy as np
 import pytest
 
+import light_cases as LC
 import oracle as O
 import pyhr
 
@@ -27,7 +28,12 @@ def compare(got, want, what):
     assert np.all(got[..., 3] == 1.0)
 
 
-@pytest.mark.parametrize("light_kw", [{}, dict(type=1, position=(4.0, 12.0, 6.0), radius=0.5, intensity=300.0)])
+# the default sun, a point light, and the spot / overhead-sun / horizon-sun / coloured cases of light_cases.py (the soft shadow-ray form
+# of the direct term: the smoothstep band, the NaN tangent of the overhead sun, N.Wi just below 0, Li per channel)
+LIGHT_KW = [{}, dict(type=1, position=(4.0, 12.0, 6.0), radius=0.5, intensity=300.0)] + [LC.BY_ID[c].kw for c in ("spot_band", "sun_overhead", "sun_horizon", "colored")]
+
+
+@pytest.mark.parametrize("light_kw", LIGHT_KW)
 def test_path_tracer_matches_the_oracle(light_kw):
     sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
