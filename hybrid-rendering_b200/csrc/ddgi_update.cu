@@ -137,10 +137,14 @@ __global__ void __launch_bounds__(256) k_sample_probe_grid(GBufLevelDev g, Frame
     const float  depth = __ldg(g.depth + idx);
     if (depth == 1.0f) { out[idx] = make_uint2(0u, 0u); return; }
     const float  u = ((float)x + 0.5f) / (float)g.W, v = ((float)y + 0.5f) / (float)g.H;
-    const float* M = fc.view_proj_inverse;
+    // world_position_from_depth (common.glsl:169-184) rounded as the reference rounds it: ((m0r*x + m1r*y) + m2r*z) + m3r, no
+    // contraction, then an IEEE division by w.  Near the far plane w = m11*depth + m15 cancels (by ~100x at near 0.1 / far 100),
+    // so fused products and an approximate reciprocal moved P far enough to change the probe visibility weights.
+    const float* M  = fc.view_proj_inverse;
     const float  sx = u * 2.0f - 1.0f, sy = v * 2.0f - 1.0f;
-    const float  iw = __fdividef(1.0f, M[3] * sx + M[7] * sy + M[11] * depth + M[15]);
-    const float3 P  = f3((M[0] * sx + M[4] * sy + M[8] * depth + M[12]) * iw, (M[1] * sx + M[5] * sy + M[9] * depth + M[13]) * iw, (M[2] * sx + M[6] * sy + M[10] * depth + M[14]) * iw);
+    auto         row = [&](int r) { return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(M[r], sx), __fmul_rn(M[4 + r], sy)), __fmul_rn(M[8 + r], depth)), M[12 + r]); };
+    const float  w  = row(3);
+    const float3 P  = f3(__fdiv_rn(row(0), w), __fdiv_rn(row(1), w), __fdiv_rn(row(2), w));
     const float2 e  = h2f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb2 + idx)));
     float3       N  = f3(e.x, e.y, 1.0f - fabsf(e.x) - fabsf(e.y));
     if (N.z < 0.0f)

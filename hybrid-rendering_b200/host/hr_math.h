@@ -50,7 +50,9 @@ inline M4 perspective(float fovy_rad, float aspect, float zn, float zf)
 {
     M4 r;
     std::memset(r.m, 0, sizeof(r.m));
-    const float t = std::tan(fovy_rad / 2.0f);
+    // tan in double, rounded once to float: the correctly rounded tangent, the value a compile-time fold of tanf gives for a
+    // constant field of view, so a field of view passed at run time reproduces the constant's bits (libm's tanf can be 1 ulp off)
+    const float t = (float)std::tan((double)(fovy_rad / 2.0f));
     r.at(0, 0)    = 1.0f / (aspect * t);
     r.at(1, 1)    = 1.0f / t;
     r.at(2, 2)    = -(zf + zn) / (zf - zn);

@@ -522,12 +522,18 @@ void hrs_default_light(hrs_light_desc* l)
 void hrs_make_frame(hr_frame* out, const float cam_pos[3], const float cam_target[3], int width, int height, const hrs_light_desc* light,
                     const hr_frame* prev, uint32_t num_frames)
 {
+    const float up[3] = { 0.0f, 1.0f, 0.0f };
+    hrs_make_frame_ex(out, cam_pos, cam_target, up, 60.0f, 1.0f, 1000.0f, width, height, light, prev, num_frames); // src/common.h:19-20
+}
+
+void hrs_make_frame_ex(hr_frame* out, const float cam_pos[3], const float cam_target[3], const float cam_up[3], float fovy_deg, float kNear,
+                       float kFar, int width, int height, const hrs_light_desc* light, const hr_frame* prev, uint32_t num_frames)
+{
     memset(out, 0, sizeof(*out));
-    const float kNear = 1.0f, kFar = 1000.0f; // src/common.h:19-20
     const float rad   = 3.14159265358979f / 180.0f;
     V3 pos = { cam_pos[0], cam_pos[1], cam_pos[2] }, tgt = { cam_target[0], cam_target[1], cam_target[2] };
-    M4 proj = perspective(60.0f * rad, (float)width / (float)height, kNear, kFar);
-    M4 view = look_at(pos, tgt, { 0, 1, 0 });
+    M4 proj = perspective(fovy_deg * rad, (float)width / (float)height, kNear, kFar);
+    M4 view = look_at(pos, tgt, { cam_up[0], cam_up[1], cam_up[2] });
     M4 vp   = mul(proj, view);
     M4 vpi = inverse(vp), vi = inverse(view), pi = inverse(proj);
     memcpy(out->ubo.view_inverse, vi.m, 64);

@@ -51,6 +51,11 @@ typedef struct hrs_light_desc {
 HR_API void hrs_default_light(hrs_light_desc* l); /* shadows-test directional preset, main.cpp:782-787 */
 HR_API void hrs_make_frame(hr_frame* out, const float cam_pos[3], const float cam_target[3], int width, int height,
                            const hrs_light_desc* light, const hr_frame* prev, uint32_t num_frames);
+/* hrs_make_frame with any camera: look_at(cam_pos, cam_target, cam_up) and perspective(fovy_deg, W/H, z_near, z_far);
+ * z_buffer_params follow z_near / z_far.  hrs_make_frame is this with up (0, 1, 0), 60 degrees, near 1, far 1000. */
+HR_API void hrs_make_frame_ex(hr_frame* out, const float cam_pos[3], const float cam_target[3], const float cam_up[3], float fovy_deg,
+                              float z_near, float z_far, int width, int height, const hrs_light_desc* light, const hr_frame* prev,
+                              uint32_t num_frames);
 
 /* Ray-cast the visible scene through frame->ubo and write mip 0 of the G-buffer (host memory):
  * gb1 RGBA8 (may be NULL), gb2/gb3 RGBA16F, depth float. */

@@ -145,6 +145,8 @@ def load_synth():
         lib.hrs_scene_world_normals.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.hrs_default_light.argtypes = [C.POINTER(hrs_light_desc)]
         lib.hrs_make_frame.argtypes = [C.POINTER(hr_frame), c_float_p, c_float_p, C.c_int, C.c_int, C.POINTER(hrs_light_desc), C.POINTER(hr_frame), C.c_uint32]
+        lib.hrs_make_frame_ex.argtypes = [C.POINTER(hr_frame), c_float_p, c_float_p, c_float_p, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int,
+                                          C.POINTER(hrs_light_desc), C.POINTER(hr_frame), C.c_uint32]
         lib.hrs_write_gbuffer.argtypes = [C.c_void_p, C.POINTER(hr_frame), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.hrs_blue_noise.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p]
         _synth = lib
@@ -289,12 +291,14 @@ def default_light(**kw):
     return l
 
 
-def make_frame(cam_pos, cam_target, W, H, prev=None, num_frames=0, light=None):
+def make_frame(cam_pos, cam_target, W, H, prev=None, num_frames=0, light=None, up=(0.0, 1.0, 0.0), fovy_deg=60.0, near=1.0, far=1000.0):
+    """hrs_make_frame_ex: look_at(cam_pos, cam_target, up), perspective(fovy_deg, W / H, near, far); the defaults are hrs_make_frame's camera"""
     f = hr_frame()
     p = (C.c_float * 3)(*cam_pos)
     t = (C.c_float * 3)(*cam_target)
-    load_synth().hrs_make_frame(C.byref(f), p, t, W, H, C.byref(light) if light is not None else None, C.byref(prev) if prev is not None else None,
-                                num_frames)
+    u = (C.c_float * 3)(*up)
+    load_synth().hrs_make_frame_ex(C.byref(f), p, t, u, fovy_deg, near, far, W, H, C.byref(light) if light is not None else None,
+                                   C.byref(prev) if prev is not None else None, num_frames)
     return f
 
 

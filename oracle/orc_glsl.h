@@ -289,6 +289,20 @@ struct ReprojectOut {
     float history_length = 0;
 };
 
+// Optional per-pixel record of the branches reproject() takes (tests only, orc_set_reproject_codes): one byte per pass pixel, the
+// ORC_RP_* bits OR-ed in.  Recording reads nothing the outputs depend on and writes nothing else.
+enum {
+    ORC_RP_REACHED  = 1,   // reproject() ran for the pixel (it has geometry)
+    ORC_RP_OUT      = 2,   // history_coord out of frame
+    ORC_RP_TRUNC    = 4,   // a history_coord_floor component in (-1, 0): ivec2() truncates it to 0 where floor gives -1
+    ORC_RP_ALL      = 8,   // bilinear, all four taps valid
+    ORC_RP_SOME     = 16,  // bilinear, one to three taps valid, sumw >= 0.01
+    ORC_RP_SUMW     = 32,  // some tap valid but sumw < 0.01: sent to the 3x3 fallback
+    ORC_RP_FALLBACK = 64,  // the 3x3 fallback found a valid texel
+    ORC_RP_VIRTUAL  = 128  // reflections: virtual-point reprojection (else the motion vector); invalid = REACHED without ALL/SOME/FALLBACK
+};
+inline uint8_t*& reproject_codes() { static uint8_t* codes = nullptr; return codes; }
+
 template <int NC>
 inline bool reproject(const ReprojectIn& in, ReprojectOut& out)
 {
@@ -327,6 +341,10 @@ inline bool reproject(const ReprojectIn& in, ReprojectOut& out)
 
     float hc[3] = { 0, 0, 0 };
     float hm[2] = { 0, 0 };
+    uint8_t code = ORC_RP_REACHED;
+    if (out_of_frame_disocclusion_check(history_coord, idim)) code |= ORC_RP_OUT;
+    if ((history_coord_floor.x > -1.0f && history_coord_floor.x < 0.0f) || (history_coord_floor.y > -1.0f && history_coord_floor.y < 0.0f)) code |= ORC_RP_TRUNC;
+    if (in.reflections && in.ray_length > 0.0f && center_g_buffer_3.y == 0.0f) code |= ORC_RP_VIRTUAL;
 
     bool        v[4];
     const ivec2 offset[4] = { { 0, 0 }, { 1, 0 }, { 0, 1 }, { 1, 1 } };
@@ -369,6 +387,7 @@ inline bool reproject(const ReprojectIn& in, ReprojectOut& out)
             }
         }
         valid = (sumw >= 0.01f); // :252
+        code |= !valid ? ORC_RP_SUMW : (v[0] && v[1] && v[2] && v[3]) ? ORC_RP_ALL : ORC_RP_SOME;
         for (int c = 0; c < NC; c++) hc[c] = valid ? hc[c] / sumw : 0.0f;
         if (in.moments)
         {
@@ -403,6 +422,7 @@ inline bool reproject(const ReprojectIn& in, ReprojectOut& out)
         if (cnt > 0)
         {
             valid = true;
+            code |= ORC_RP_FALLBACK;
             for (int c = 0; c < NC; c++) hc[c] /= cnt;
             if (in.moments)
             {
@@ -425,6 +445,7 @@ inline bool reproject(const ReprojectIn& in, ReprojectOut& out)
     for (int c = 0; c < 3; c++) out.history_color[c] = hc[c];
     out.history_moments[0] = hm[0];
     out.history_moments[1] = hm[1];
+    if (uint8_t* codes = reproject_codes()) codes[(size_t)frag_coord.y * idim.x + frag_coord.x] = code;
     return valid;
 }
 

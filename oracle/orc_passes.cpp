@@ -473,6 +473,9 @@ void build_mip(int W, int H, const uint16_t* gb2, const uint16_t* gb3, const flo
 // ================================================================================================
 extern "C" {
 
+// record reproject()'s branches (ORC_RP_* bits, orc_glsl.h) into `codes` (one byte per pixel of the next temporal stage's pass), or stop (NULL)
+void orc_set_reproject_codes(uint8_t* codes) { reproject_codes() = codes; }
+
 struct orc_gbuf { int32_t W, H; const uint16_t* gb2; const uint16_t* gb3; const float* depth; };
 static GBufLevel lvl(const orc_gbuf* g) { GBufLevel l; l.W = g->W; l.H = g->H; l.gb2 = g->gb2; l.gb3 = g->gb3; l.depth = g->depth; return l; }
 

@@ -82,6 +82,7 @@ def lib():
         L.orc_fetch_normal.argtypes = [P, P, P, C.c_size_t, I, P]
         L.orc_texture_sample.argtypes = [P, P, C.c_size_t, P]
         L.orc_fetch_material.argtypes = [P, P, P, C.c_size_t, P]
+        L.orc_set_reproject_codes.argtypes = [P]
         _lib = L
     return _lib
 
@@ -318,6 +319,32 @@ class AOOracle:
             L.orc_upsample_scalar(C.byref(g0), C.byref(gc), p(self.blur[1]), 1, 1.0, P.power, p(self.upsample))
             self._poison(self.upsample, 0, shift=self.scale)
             self.final = self.upsample
+
+
+# reproject()'s branch bits (oracle/orc_glsl.h ORC_RP_*); "invalid" is a reached pixel with none of all / some / fallback
+RP_BITS = {"reached": 1, "out": 2, "trunc": 4, "all": 8, "some": 16, "sumw": 32, "fallback": 64, "virtual": 128}
+
+
+class ReprojectCodes:
+    """`with ReprojectCodes(W, H) as rc:` around one temporal stage (K3, K9 or K14) records the branch reproject() takes at every pixel
+    of that W x H pass in rc.codes; rc.counts() -> {branch: pixel count}.  The stage's outputs are unchanged."""
+
+    def __init__(self, W, H):
+        self.codes = np.zeros((H, W), np.uint8)
+
+    def __enter__(self):
+        lib().orc_set_reproject_codes(p(self.codes))
+        return self
+
+    def __exit__(self, *exc):
+        lib().orc_set_reproject_codes(None)
+
+    def counts(self):
+        c = self.codes
+        out = {k: int(np.count_nonzero(c & b)) for k, b in RP_BITS.items()}
+        out["invalid"] = int(np.count_nonzero((c & 1) & ((c & (8 | 16 | 64)) == 0)))
+        out["motion"] = out["reached"] - out["virtual"]
+        return out
 
 
 def h2f(a):

@@ -78,9 +78,12 @@ def new_context(sc, W, H):
     return ctx
 
 
-def same_gbuffer(ctx, f, ref: O.GBufMips, W, H):
-    """the device G-buffer producer and its mips 1 and 2 are the oracle's bits; the frame is not all sky (1x1 and 7x3 included)"""
+def same_gbuffer(ctx, f, ref: O.GBufMips, W, H, gb1=None):
+    """the device G-buffer producer and its mips 1 and 2 are the oracle's bits; the frame is not all sky (1x1 and 7x3 included).
+    gb1: the oracle's albedo / metallic image, compared at mip 0 (the mip chain carries gb2, gb3 and depth only)"""
     assert (ref.levels[0][4] != 1.0).any(), f"{W}x{H}: the camera sees no geometry"
+    if gb1 is not None:
+        assert np.array_equal(ctx.gbuffer_download(f.ping_pong, 0, 1, W, H), gb1), f"{W}x{H}: device G-buffer image 1 of mip 0 differs"
     for mip in range(3):
         _, _, gb2, gb3, depth = ref.levels[mip]
         for which, arr in ((0, depth), (2, gb2), (3, gb3)):
@@ -105,7 +108,9 @@ def measure_sh_ao(w, sh, ao, osh, oao):
 
 
 def run_shadows_ao(case, W, H, sh_scale, ao_scale, sh_params=None, ao_params=None, n=5, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0,
-                   cam=CAM_SHADOWS_TEST, light=None, check=check_all, pan_from=3):
+                   cam=CAM_SHADOWS_TEST, light=None, check=check_all, pan_from=3, seq=None, before=None, after=None):
+    """seq: the (i, frame) sequence to run in place of frames(W, H, n, pan_from, vertical, cam, light); before(i, f, (sh, ao), (osh, oao))
+    runs before frame i's renders (a history reset), after(i, f, cur_g, prev_g, (sh, ao), (osh, oao)) after its comparisons"""
     sc = pyhr.SynthScene(scene, tris)
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
@@ -116,20 +121,25 @@ def run_shadows_ao(case, W, H, sh_scale, ao_scale, sh_params=None, ao_params=Non
     set_params([ao.params, oao.params], ao_params)
     w = Worst(case)
     prev_g = O.zero_gbuf_mips(W, H)
-    for i, f in frames(W, H, n, pan_from, vertical, cam, light):
+    for i, f in (seq if seq is not None else frames(W, H, n, pan_from, vertical, cam, light)):
+        if before:
+            before(i, f, (sh, ao), (osh, oao))
         ctx.gbuffer_render(f.ping_pong, f)
-        cur_g = O.GBufMips(O.gbuffer_render(ss, f, W, H))
-        same_gbuffer(ctx, f, cur_g, W, H)
+        g = O.gbuffer_render(ss, f, W, H)
+        cur_g = O.GBufMips(g)
+        same_gbuffer(ctx, f, cur_g, W, H, g.gb1)
         sh.render(f)
         ao.render(f)
         osh.render(ss.scene, cur_g, prev_g, f, bn)
         oao.render(ss.scene, cur_g, prev_g, f, bn)
-        prev_g = cur_g
         if check is check_all:
             check_all(i, sh, ao, osh, oao, [])
         else:
             check(i, sh, ao, osh, oao)
         measure_sh_ao(w, sh, ao, osh, oao)
+        if after:
+            after(i, f, cur_g, prev_g, (sh, ao), (osh, oao))
+        prev_g = cur_g
     w.report()
     sh.destroy()
     ao.destroy()
@@ -192,14 +202,15 @@ def check_ddgi(i, dd, odd, w, cmp=close):
 
 
 def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0, cam=CAM_SHADOWS_TEST,
-                light=None, ddgi_params=None, lut=None, ddgi_hook=None, frame_hook=None, cmp=close):
+                light=None, ddgi_params=None, lut=None, ddgi_hook=None, frame_hook=None, cmp=close, seq=None, before=None, after=None):
     """test_gpu_gi_refl.run at any size and scale (DDGI sampled at the reflections' scale), fed by the device G-buffer producer.
     ddgi_params: overrides of the DDGI parameter block; lut: a BRDF LUT set on the context and the oracle (the reflections' IBL
     specular term, as in test_deferred); ddgi_hook(i, f, rot, dd, odd, fresh) runs before frame i's DDGI render and returns the
     DDGI oracle to go on with (fresh() makes a new one from dd.params: a re-initialised grid); frame_hook(i, dd, odd, rf, orf) runs
     after frame i's comparisons.  cmp: the comparison of the DDGI and reflections images (`close`, or a rule with its signature; a
     rule that sets cmp.stopped ends the run after the comparison that set it).
-    scene: a SynthScene kind, or an object with SynthScene's interface"""
+    scene: a SynthScene kind, or an object with SynthScene's interface.  seq, before(i, f, (dd, rf), (odd, orf)) and
+    after(i, f, cur_g, prev_g, (dd, rf), (odd, orf)): as in run_shadows_ao (after runs once the denoised images are compared)"""
     sc = pyhr.SynthScene(scene, tris) if isinstance(scene, int) else scene
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
@@ -226,10 +237,13 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
         orf.brdf_lut = lut
     w = Worst(case)
     prev_g = O.zero_gbuf_mips(W, H)
-    for i, f in frames(W, H, n, pan_from, vertical, cam, light):
+    for i, f in (seq if seq is not None else frames(W, H, n, pan_from, vertical, cam, light)):
+        if before:
+            before(i, f, (dd, rf), (odd, orf))
         ctx.gbuffer_render(f.ping_pong, f)
-        cur_g = O.GBufMips(O.gbuffer_render(ss, f, W, H))
-        same_gbuffer(ctx, f, cur_g, W, H)
+        g = O.gbuffer_render(ss, f, W, H)
+        cur_g = O.GBufMips(g)
+        same_gbuffer(ctx, f, cur_g, W, H, g.gb1)
         if dd:
             rot = pyhr.rotation_matrix(0.7 + 1.3 * i, (0.3, 1.0, -0.5))
             if ddgi_hook:
@@ -241,7 +255,6 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
                 break
         rf.render(f, dd)
         orf.render(ss, cur_g, prev_g, f, bn, odd)
-        prev_g = cur_g
         rt_c, rt_o = f16(rf.download(0)), O.h2f(orf.rt)
         assert np.array_equal(rt_c[..., 3], rt_o[..., 3]), f"frame {i}: reflection ray length (hit / miss / t) not exact"
         cmp(rt_c[..., :3], rt_o[..., :3], f"frame {i} reflections ray trace", 1e-3, 0.02)
@@ -249,6 +262,7 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
         if not rf.params.denoise:
             if frame_hook:
                 frame_hook(i, dd, odd, rf, orf)
+            prev_g = cur_g
             continue
         assert np.array_equal(rf.download(6), orf.tile_flags), f"frame {i}: reflections tile classification"
         mo_c, mo_o = f16(rf.download(4)), O.h2f(orf.cur_moments)
@@ -259,6 +273,9 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
             w.add(name, got, want)
         if frame_hook:
             frame_hook(i, dd, odd, rf, orf)
+        if after:
+            after(i, f, cur_g, prev_g, (dd, rf), (odd, orf))
+        prev_g = cur_g
     w.report()
     rf.destroy()
     if dd:
