@@ -291,10 +291,10 @@ inline int hr_rt_share_cap(int MH, int world) { const int c = 2 * ((MH + world -
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out); // false when the pass is not linked to peers
 int  hr_rt_share_finish(hr_pass* p, int parity, int tick, cudaStream_t st); // push costs, signal the ray-trace tick
 int  hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cudaStream_t st); // wait for the peers' ticks, then next frame's bounds
-// Interleaved cooperative ray trace of the reflections pass (shard.cu): rank r traces the 8-row chunks c with c % world == r of the
+// Interleaved cooperative ray trace of the reflections pass and the path tracer (shard.cu): rank r traces the 8-row chunks c with c % world == r of the
 // WHOLE image into its own image and copies every chunk to the ranks whose denoise stages read it (rows [need0[q], need1[q]));
 // the last block publishes the ray-trace tick.
-int hr_refl_push_chunks(hr_pass* p, int parity, int tick, const int* need0, const int* need1, cudaStream_t st);
+int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* need1, cudaStream_t st); // img: the shared image (hr_peer_register index)
 // Rows of an image of height H owned by this context's rank (all rows when world == 1).
 void hr_band(const hr_ctx* ctx, int H, int* b0, int* b1);
 // [b0 - halo, b1 + halo) clamped to [0, H); halo must be a multiple of 8 so tile alignment is kept.
@@ -320,12 +320,13 @@ void launch_deferred(const GBufLevelDev& g, const FrameConsts& fc, const void* s
                      const float* env3, const void* brdf_lut, void* out, int row0, int row1, cudaStream_t st); // deferred.cu
 // rt_shade.cu: ground-truth path tracer
 void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, cudaStream_t st);
-// post.cu
+                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, int row0, int row1,
+                       int chunk_first, int chunk_stride, cudaStream_t st); // rows [row0, row1), or chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride
+// post.cu: TAA and tone map resolve rows [row0, row1); the blit covers the whole image
 void launch_taa(const GBufLevelDev& g, const void* current, int current_channels, const void* history, const float* jitter_xy, float feedback_min, float feedback_max,
-                int sharpen, void* out, cudaStream_t st);
+                int sharpen, void* out, int row0, int row1, cudaStream_t st);
 void launch_blit_rgba16f(const void* src, int channels, int W, int H, void* out, cudaStream_t st);
-void launch_tonemap(const void* src, int channels, int W, int H, float exposure, int single_channel, void* out_rgba8, cudaStream_t st);
+void launch_tonemap(const void* src, int channels, int W, int H, float exposure, int single_channel, void* out_rgba8, int row0, int row1, cudaStream_t st);
 // stats.cu (measurement helpers, not on the frame path)
 void launch_tile_stats(const uint8_t* flags, int TW, int t0, int t1, unsigned long long* d_out, cudaStream_t st);
 void launch_drain_ray_counters(unsigned long long* ctr, unsigned long long* d_out, cudaStream_t st);

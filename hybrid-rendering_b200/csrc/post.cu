@@ -15,10 +15,11 @@ namespace {
 
 using namespace post;
 
-__global__ void __launch_bounds__(256) k_taa(TaaArgs A, uint2* __restrict__ out)
+// rows [row0, row1): a sharded rank resolves its band (the inputs it reads are complete on every rank, hr_taa_render)
+__global__ void __launch_bounds__(256) k_taa(TaaArgs A, int row0, int row1, uint2* __restrict__ out)
 {
-    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (x >= A.W || y >= A.H) return;
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (x >= A.W || y >= row1) return;
     const F4 c = taa_pixel(A, x, y);
     out[(size_t)y * A.W + x] = make_uint2((uint32_t)float_to_half_bits(c.x) | ((uint32_t)float_to_half_bits(c.y) << 16),
                                           (uint32_t)float_to_half_bits(c.z) | ((uint32_t)float_to_half_bits(c.w) << 16));
@@ -34,10 +35,10 @@ __global__ void __launch_bounds__(256) k_blit_rgba16f(ImgView src, uint2* __rest
                                             (uint32_t)float_to_half_bits(c.z) | ((uint32_t)float_to_half_bits(c.w) << 16));
 }
 
-__global__ void __launch_bounds__(256) k_tonemap(ImgView src, float exposure, int single_channel, uint32_t* __restrict__ out)
+__global__ void __launch_bounds__(256) k_tonemap(ImgView src, float exposure, int single_channel, int row0, int row1, uint32_t* __restrict__ out)
 {
-    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (x >= src.W || y >= src.H) return;
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (x >= src.W || y >= row1) return;
     out[(size_t)y * src.W + x] = tonemap_pixel(fetch_texel(src, x, y), exposure, single_channel);
 }
 
@@ -51,8 +52,9 @@ ImgView view(const void* p, int W, int H, int channels)
 } // namespace
 
 void launch_taa(const GBufLevelDev& g, const void* current, int current_channels, const void* history, const float* jitter_xy, float feedback_min, float feedback_max,
-                int sharpen, void* out, cudaStream_t st)
+                int sharpen, void* out, int row0, int row1, cudaStream_t st)
 {
+    if (row1 <= row0) return;
     TaaArgs A;
     A.cur   = view(current, g.W, g.H, current_channels);
     A.prev  = view(history, g.W, g.H, 4);
@@ -63,8 +65,8 @@ void launch_taa(const GBufLevelDev& g, const void* current, int current_channels
     A.jitter_x = jitter_xy[0]; A.jitter_y = jitter_xy[1];
     A.feedback_min = feedback_min; A.feedback_max = feedback_max;
     A.sharpen = sharpen;
-    dim3 grid((g.W + 31) / 32, (g.H + 7) / 8);
-    k_taa<<<grid, 256, 0, st>>>(A, (uint2*)out);
+    dim3 grid((g.W + 31) / 32, (row1 - row0 + 7) / 8);
+    k_taa<<<grid, 256, 0, st>>>(A, row0, row1, (uint2*)out);
 }
 
 void launch_blit_rgba16f(const void* src, int channels, int W, int H, void* out, cudaStream_t st)
@@ -73,8 +75,9 @@ void launch_blit_rgba16f(const void* src, int channels, int W, int H, void* out,
     k_blit_rgba16f<<<grid, 256, 0, st>>>(view(src, W, H, channels), (uint2*)out);
 }
 
-void launch_tonemap(const void* src, int channels, int W, int H, float exposure, int single_channel, void* out_rgba8, cudaStream_t st)
+void launch_tonemap(const void* src, int channels, int W, int H, float exposure, int single_channel, void* out_rgba8, int row0, int row1, cudaStream_t st)
 {
-    dim3 grid((W + 31) / 32, (H + 7) / 8);
-    k_tonemap<<<grid, 256, 0, st>>>(view(src, W, H, channels), exposure, single_channel, (uint32_t*)out_rgba8);
+    if (row1 <= row0) return;
+    dim3 grid((W + 31) / 32, (row1 - row0 + 7) / 8);
+    k_tonemap<<<grid, 256, 0, st>>>(view(src, W, H, channels), exposure, single_channel, row0, row1, (uint32_t*)out_rgba8);
 }

@@ -387,6 +387,7 @@ struct PathTraceParams {
     float    sky[3];
     int      W, H;
     unsigned long long* ray_ctr;
+    int      row0, row1, chunk_first, chunk_stride; // chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
 };
 
 __device__ __forceinline__ float4 mat_vec4(const float* M, float x, float y, float z, float w)
@@ -478,8 +479,11 @@ __global__ void __launch_bounds__(64) k_path_trace(BvhDev bvh, ShadeDev sd, Path
                                                    tex::TexDev T, uint32_t* __restrict__ out_hash)
 {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int x = blockIdx.x * 16 + warp * 8 + (lane & 7), y = blockIdx.y * 4 + (lane >> 3);
-    if (x >= P.W || y >= P.H) return;
+    // rows: [row0, row1) or, when the ranks trace cooperatively, the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
+    // (the row mapping of k_reflections_ray_trace).  The RNG is seeded from (x, y, sample): no result depends on the rank.
+    const int x = blockIdx.x * 16 + warp * 8 + (lane & 7);
+    const int y = (P.chunk_stride > 1 ? 8 * (P.chunk_first + ((int)blockIdx.y >> 1) * P.chunk_stride) + 4 * ((int)blockIdx.y & 1) : P.row0 + (int)blockIdx.y * 4) + (lane >> 3);
+    if (x >= P.W || y >= P.H || (P.chunk_stride <= 1 && y >= P.row1)) return;
     const size_t idx = (size_t)y * P.W + x;
     // rgen:56-75
     gi::RNG     rng = gi::rng_init((uint32_t)x, (uint32_t)y, P.num_frames);
@@ -621,8 +625,11 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
 }
 
 void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, cudaStream_t st)
+                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, int row0, int row1,
+                       int chunk_first, int chunk_stride, cudaStream_t st)
 {
+    const int n_chunks_mine = chunk_stride > 1 ? (((H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0;
+    if (chunk_stride > 1 ? n_chunks_mine <= 0 : row1 <= row0) return;
     PathTraceParams P;
     memcpy(P.view_inverse, f->ubo.view_inverse, 64);
     memcpy(P.proj_inverse, f->ubo.proj_inverse, 64);
@@ -631,7 +638,8 @@ void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint
     P.sky[0] = sky3[0]; P.sky[1] = sky3[1]; P.sky[2] = sky3[2];
     P.W = W; P.H = H;
     P.ray_ctr = ray_ctr;
-    dim3 grid((W + 15) / 16, (H + 3) / 4);
+    P.row0 = row0; P.row1 = row1; P.chunk_first = chunk_first; P.chunk_stride = chunk_stride;
+    dim3 grid((W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
 #define HR_PT_ARGS hr_bvh_view(sc), shade_view(sc), P, (const uint2*)prev, (uint2*)out, out_prim, sc->tex
     const bool textured = sc->tex.n_textures > 0; // material textures change the lobe inputs: both indirect forms have a TEX instantiation
     if (trace_indirect)

@@ -309,8 +309,9 @@ __global__ void k_peer_wait(const int* __restrict__ ticks, int world, int self, 
     }
 }
 
-// Reflections (interleaved cooperative ray trace): block b copies this rank's chunk c = self + b * world (8 image rows of RGBA16F
-// texels) to every rank whose denoise stages read those rows; the last block to finish publishes the ray-trace tick.
+// Interleaved cooperative ray trace (reflections, path tracer): block b copies this rank's chunk c = self + b * world (8 image rows of
+// RGBA16F texels) to every rank that reads those rows; the last block to finish publishes the ray-trace tick.  A rank that owns no
+// chunk still runs PUSH_SPLIT blocks so that its tick is published.
 #define PUSH_SPLIT 4
 struct RowPtrs { uint2* p[HR_MAX_RANKS]; };
 struct NeedRows { int r0[HR_MAX_RANKS], r1[HR_MAX_RANKS]; };
@@ -485,7 +486,7 @@ int hr_peer_signal(hr_pass* p, int which, int tick, cudaStream_t st)
     return HR_OK;
 }
 
-int hr_refl_push_chunks(hr_pass* p, int parity, int tick, const int* need0, const int* need1, cudaStream_t st)
+int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* need1, cudaStream_t st)
 {
     hr_ctx* ctx = p->ctx;
     RowPtrs  im {};
@@ -493,7 +494,7 @@ int hr_refl_push_chunks(hr_pass* p, int parity, int tick, const int* need0, cons
     TickPtrs t {};
     for (int r = 0; r < ctx->world; r++)
     {
-        im.p[r]  = static_cast<uint2*>(p->hist_peer[r][4 + parity]);
+        im.p[r]  = static_cast<uint2*>(p->hist_peer[r][img]);
         nd.r0[r] = need0[r];
         nd.r1[r] = need1[r];
         t.p[r]   = p->peer_ticks[r];

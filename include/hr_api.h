@@ -440,8 +440,13 @@ HR_API int hr_deferred_render(hr_pass* pass, const hr_frame* frame, const hr_def
  * Post-processing  (SURVEY.md §8 f4: src/temporal_aa.{h,cpp} + shaders/taa.comp; src/tone_map.{h,cpp} + shaders/tone_map.frag)
  * Both passes read the FINAL output (which = 100) of any other pass at full resolution — the reference binds the deferred,
  * shadows, AO, reflections or DDGI output by visualisation type (temporal_aa.cpp:136-147, tone_map.cpp:106-125); R16F / RG16F
- * inputs are read as (r, 0, 0, 1) / (r, g, 0, 1) like a sampler does.  Not sharded: with world > 1 run them on a rank that holds
- * the gathered outputs (hr_shard_set_gather) and a complete G-buffer.
+ * inputs are read as (r, 0, 0, 1) / (r, g, 0, 1) like a sampler does.
+ * Sharded (world > 1): each rank resolves / maps its band hr_shard_rows(H).  TAA reads the input's 3x3 neighbourhood one row beyond
+ * the band and its own previous output wherever the motion vector reprojects it, so it needs complete inputs: the input pass's
+ * gathered final output, the G-buffer rows of the band + 2 (the sharded G-buffer's halo covers them) and its own output, which it
+ * gathers after every render (8 B/px).  With world > 1 and the gather off (hr_shard_set_gather(ctx, 0)) hr_taa_render returns
+ * HR_ERR_UNSUPPORTED and changes nothing.  Its reset blit copies the whole gathered input on every rank.  The tone map reads only its
+ * band of the input and gathers its RGBA8 output (4 B/px) when the gather is on; with the gather off each rank holds its band only.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct hr_taa_params { /* defaults: src/temporal_aa.h:54-59 */
     float   feedback_min;      /* 0.88 */
@@ -479,7 +484,15 @@ HR_API int hr_tonemap_render(hr_pass* pass, const hr_tonemap_params* params, hr_
  * sample (each with its shadow ray); running average over renders.  As written in the reference the indirect bounce is disabled
  * (its traceRayEXT is commented out, ground_truth_path_trace.rchit:92-104), so max_ray_bounces changes nothing unless trace_indirect
  * is 1.  Needs only the
- * scene and frame->ubo.{view_inverse, proj_inverse, light}: no G-buffer.  Replicated (not sharded) when world > 1.
+ * scene and frame->ubo.{view_inverse, proj_inverse, light}: no G-buffer.
+ * Sharded (world > 1): linked to its peers (hr_shard_init, or hr_shard_link_local for ranks of one process) rank r traces the 8-row
+ * chunks c with c % world == r of the whole image; with only hr_shard_config it traces its band hr_shard_rows(H).  A rank's running
+ * average covers its own rows, which are bit for bit the single-GPU rows; its ray counters (hr_pass_get_stats) count its own rows, the
+ * ranks' counts sum to the single-GPU counts.  With the gather on (the default) a linked rank pushes its chunks into every peer's
+ * image and its render ends with a wait on `stream` for every peer's chunks of that render: FINAL / COLOR are then complete on every
+ * rank.  Consumers of the output must run on the render stream.  The gather needs an even width: an odd one returns HR_ERR_UNSUPPORTED
+ * and changes nothing.  With the gather off FINAL / COLOR hold the rank's own rows only; PRIMITIVE and PATH_HASH always do.
+ * hr_pass_reset_history must be called on all ranks together.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct hr_path_tracer_params {
     int32_t max_ray_bounces;      /* 2 (ground_truth_path_tracer.h:28; the ctor overwrites it with the device's recursion limit) */
