@@ -711,7 +711,8 @@ struct PassAllocs {
     void operator()(T*& ptr, size_t count, int fill_byte = 0) { if (rc == HR_OK) rc = pass_alloc(p, ptr, count, fill_byte); }
 };
 
-// multi-GPU ray-trace sharing (shard.cu): second ray-mask image (frame parity), cost tables, device-side row partition
+// multi-GPU ray-trace sharing (shard.cu): second ray-mask image (frame parity), cost tables, device-side row partition.  The two
+// spp > 1 count images of the cooperative trace are allocated when the pass is linked (rt_alloc_counts, shard.cu).
 static void pass_alloc_rt_share(PassAllocs& A)
 {
     hr_pass*     p  = A.p;
@@ -854,23 +855,25 @@ static_assert((int)HR_SHADOWS_OUT_RAY_TRACE == (int)HR_AO_OUT_RAY_TRACE && (int)
 
 // ray_trace (ray_traced_shadows.cpp:972-1011, ray_traced_ao.cpp:864-903): K1 (p0 = bias) or K7 (p0 = ray length, p1 = bias) into
 // the mask image, or with spp > 1 into the count image, then the wait for last frame's history if the temporal stage reads it.
-// Linked to peers (spp = 1): this rank traces its cost-balanced share of the WHOLE image and stores the mask words into every
-// rank's mask image (no halo re-trace); otherwise its band +- the ray-trace halo into its own image.
+// Linked to peers: this rank traces its cost-balanced share of the WHOLE image and stores the mask words (spp > 1: the counts) into
+// every rank's image of this frame's parity (no halo re-trace); otherwise its band +- the ray-trace halo into its own image.
 static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const FrameConsts& fc, float p0, float p1, int spp, bool denoise, uint32_t** mask_out,
-                      bool* shared_out)
+                      uint8_t** count_out, bool* shared_out)
 {
     hr_ctx*      ctx    = p->ctx;
     const int    parity = fr.epoch & 1;
     const BvhDev bvh    = hr_bvh_view(ctx->scene);
     RtShare      rts;
-    const bool   shared = spp == 1 && hr_rt_share(p, parity, &rts);
+    const bool   shared = hr_rt_share(p, parity, &rts);
     uint32_t*    mask   = shared ? p->mask_pp[parity] : p->mask;
+    uint8_t*     count  = shared ? p->count_pp[parity] : p->count;
     int          rc;
     if (shared)
     {
-        launch_ray_trace_mask_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, rts, fr.st);
+        if (spp > 1) launch_ray_trace_count_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), count, spp, rts, fr.st);
+        else launch_ray_trace_mask_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, rts, fr.st);
         ctx->launches++;
-        if ((rc = hr_rt_share_finish(p, parity, fr.epoch, fr.st)) != HR_OK) return rc;
+        if ((rc = hr_rt_share_finish(p, parity, fr.epoch, spp > 1, fr.st)) != HR_OK) return rc;
         timer_mark(p, "Ray Trace", fr.st);
         // every rank's share of this frame's mask (and cost table) has arrived and, when the temporal stage reads it, last frame's
         // history is complete: this wait also covers the history tick, so the temporal stage does not wait on it again
@@ -882,7 +885,8 @@ static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const 
         if (spp > 1)
         { // SURVEY.md §8d: spp rays per pixel into an 8-bit count image (allocated on first use)
             if (!p->count && (rc = pass_alloc(p, p->count, (size_t)p->W * p->H)) != HR_OK) return rc;
-            launch_ray_trace_count(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), p->count, spp, fr.rt0, fr.rt1, fr.st);
+            count = p->count;
+            launch_ray_trace_count(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), count, spp, fr.rt0, fr.rt1, fr.st);
         }
         else launch_ray_trace_mask(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, mask, fr.rt0, fr.rt1, fr.st);
         ctx->launches++;
@@ -891,10 +895,11 @@ static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const 
         // peer has finished writing them (tick epoch - 1), overlapped with the ray trace above
         if (denoise && !fr.no_history && (rc = hr_peer_wait(p, 0, fr.epoch - 1, fr.st)) != HR_OK) return rc;
     }
-    if (spp > 1) fr.final = { p->count, p->W, p->H, HR_FMT_R8_UINT };
+    if (spp > 1) fr.final = { count, p->W, p->H, HR_FMT_R8_UINT };
     else fr.final = { mask, (p->W + 7) / 8, (p->H + 3) / 4, HR_FMT_R32_UINT };
     p->out_view[HR_SHADOWS_OUT_RAY_TRACE] = fr.final;
     *mask_out   = mask;
+    *count_out  = count;
     *shared_out = shared;
     return HR_OK;
 }
@@ -948,8 +953,8 @@ int hr_shadows_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** o
         A(p->tile_flags, tw * th);
         if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
         pass_alloc_rt_share(A);
-        void* hist[7] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
-        hr_peer_register(p, hist, 7);
+        void* hist[9] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all, p->count_pp[0], p->count_pp[1] };
+        hr_peer_register(p, hist, 9);
         for (int i = 0; i < 2; i++)
         {
             p->hist_view[HR_SHADOWS_OUT_PREV_IMAGE][i] = { p->prev_image[i], p->W, p->H, HR_FMT_RG16F };
@@ -986,8 +991,9 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
         p->first = false; // nothing below reads it (unlike reflections)
     }
     uint32_t* mask;
+    uint8_t*  count;
     bool      shared_rt;
-    if ((rc = trace_mask(p, fr, cur, fc, prm->bias, 0.0f, spp, prm->denoise != 0, &mask, &shared_rt)) != HR_OK) return rc;
+    if ((rc = trace_mask(p, fr, cur, fc, prm->bias, 0.0f, spp, prm->denoise != 0, &mask, &count, &shared_rt)) != HR_OK) return rc;
     if (prm->denoise)
     {
         // temporal_accumulation (:1041-1090); reset_args (:1015-1037) is subsumed by the per-tile flag image.
@@ -995,7 +1001,7 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
         HistPeers hist;
         hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
         if (spp > 1)
-            launch_shadows_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
+            launch_shadows_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
         else
             launch_shadows_temporal(cur, prev, mask, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;
@@ -1083,8 +1089,8 @@ int hr_ao_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** out)
         A(p->tile_flags, tw * th);
         if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
         pass_alloc_rt_share(A);
-        void* hist[7] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all };
-        hr_peer_register(p, hist, 7);
+        void* hist[9] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all, p->count_pp[0], p->count_pp[1] };
+        hr_peer_register(p, hist, 9);
         for (int i = 0; i < 2; i++)
         {
             p->hist_view[HR_AO_OUT_TEMPORAL_ACCUMULATION][i] = { p->ao_color[i], p->W, p->H, HR_FMT_R16F };
@@ -1117,14 +1123,15 @@ int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* s
         p->first = false;
     }
     uint32_t* mask;
+    uint8_t*  count;
     bool      shared_rt;
-    if ((rc = trace_mask(p, fr, cur, fc, prm->ray_length, prm->bias, spp, prm->denoise != 0, &mask, &shared_rt)) != HR_OK) return rc;
+    if ((rc = trace_mask(p, fr, cur, fc, prm->ray_length, prm->bias, spp, prm->denoise != 0, &mask, &count, &shared_rt)) != HR_OK) return rc;
     if (prm->denoise)
     {
         // history = ao_color[!pp] / ao_len[!pp] of the rank that owns the reprojected row (peer history, shard.cu)
         HistPeers hist;
         hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
-        if (spp > 1) launch_ao_temporal_count(cur, prev, p->count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
+        if (spp > 1) launch_ao_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         else launch_ao_temporal(cur, prev, mask, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;
         if ((rc = frame_signal(p, fr)) != HR_OK) return rc; // this frame's history (ao_color[pp], ao_len[pp]) is complete

@@ -56,7 +56,7 @@ struct FrameConsts {           // what kernels need from hr_frame (passed by val
 
 // ---- objects ----------------------------------------------------------------------------------------
 #define HR_MAX_RANKS 8
-#define HR_MAX_SHARED 8
+#define HR_MAX_SHARED 9
 
 // Temporal history as the reprojection kernels see it (shard.cu, "peer history").  Row y of the previous frame's history
 // images lives on the rank that owns y (band_end[r] = first row NOT owned by ranks 0..r); img[r] / aux[r] are that rank's
@@ -183,7 +183,7 @@ struct hr_pass {
     Img     hist_view[8][2];   // history surfaces by `which` (< 8) and frame parity, known from creation: hr_pass_upload before the first render
     // shadows
     uint32_t* mask = nullptr;
-    uint8_t*  count = nullptr;       // spp > 1: unoccluded rays per pixel (allocated on first use)
+    uint8_t*  count = nullptr;       // spp > 1: unoccluded rays per pixel (allocated on first use; linked ranks use count_pp)
     __half2*  temporal_out = nullptr;
     uint2*    moments[2] = { nullptr, nullptr };
     __half2*  prev_image[2] = { nullptr, nullptr }; // [ping_pong]: written by frame N's feedback iteration, read by frame N+1's temporal
@@ -231,11 +231,12 @@ struct hr_pass {
     // "rank q finished writing frame N's history" before "rank r's frame N+1 reprojection reads it"
     bool        peers_linked = false, peers_ipc = false;
     int         n_hist = 0;                          // shared images: 0-3 history (shadows: prev_image[2], moments[2]; AO: colour[2], length[2]),
-                                                     // 4-5 ray mask [frame parity], 6 ray-trace cost table [2][mask rows]
+                                                     // 4-5 ray mask [frame parity], 6 ray-trace cost table [2][mask rows], 7-8 count image [frame parity] (null until linked)
     void*       hist_local[HR_MAX_SHARED] = {};
     void*       hist_peer[HR_MAX_RANKS][HR_MAX_SHARED] = {}; // [rank][image]; own rank = hist_local
     int*        sync_ticks = nullptr;                // [2][HR_MAX_RANKS] ticks written by the peers into THIS rank's memory: [0] history, [1] ray trace
     uint32_t*   mask_pp[2] = { nullptr, nullptr };   // ray mask by frame parity (mask_pp[0] == mask); peers push their rows into both copies' owner
+    uint8_t*    count_pp[2] = { nullptr, nullptr };  // spp > 1 on linked ranks: the count image by frame parity, pushed like mask_pp (allocated at link time)
     uint32_t*   rt_cost_all = nullptr;               // [2][MH] per-mask-row trace cost of the frame (all ranks' rows, pushed by their owners)
     uint32_t*   rt_cost_acc = nullptr;               // [MH] this rank's accumulation scratch (atomicAdd per warp), drained by the push kernel
     int*        rt_bounds = nullptr;                 // [world+1] mask-row partition of the NEXT frame's ray trace (device side, cost balanced); [HR_MAX_RANKS+1] = job counter, [+2] = push blocks done
@@ -289,7 +290,7 @@ struct RtShare {
 // most mask rows one rank may be handed: twice the uniform share (+4); the whole image for world <= 2
 inline int hr_rt_share_cap(int MH, int world) { const int c = 2 * ((MH + world - 1) / world) + 4; return c < MH ? c : MH; }
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out); // false when the pass is not linked to peers
-int  hr_rt_share_finish(hr_pass* p, int parity, int tick, cudaStream_t st); // push costs, signal the ray-trace tick
+int  hr_rt_share_finish(hr_pass* p, int parity, int tick, bool count, cudaStream_t st); // push the share (mask rows, or count rows when `count`) and costs, signal the ray-trace tick
 int  hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cudaStream_t st); // wait for the peers' ticks, then next frame's bounds
 // Interleaved cooperative ray trace of the reflections pass and the path tracer (shard.cu): rank r traces the 8-row chunks c with c % world == r of the
 // WHOLE image into its own image and copies every chunk to the ranks whose denoise stages read it (rows [need0[q], need1[q]));
@@ -354,11 +355,13 @@ void launch_shadows_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& 
 void launch_ao_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
                               float alpha, __half* out, __half* len_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 // trace.cu: the shadows (kind PASS_SHADOWS, K1: p0 = bias) and AO (PASS_AO, K7: p0 = ray length, p1 = bias) ray traces into the mask image,
-// the mask images of the cooperative trace (shard.cu) or, spp > 1, the count image
+// the mask images of the cooperative trace (shard.cu) or, spp > 1, the count image (band-local or cooperative)
 void launch_ray_trace_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
                            uint32_t* mask, int row0, int row1, cudaStream_t st);
 void launch_ray_trace_mask_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
                                   const uint8_t* sr, const RtShare& sh, cudaStream_t st);
+void launch_ray_trace_count_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
+                                   const uint8_t* sr, uint8_t* count, int spp, const RtShare& sh, cudaStream_t st);
 void launch_ray_trace_count(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
                             uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
 void launch_trace_any(const BvhDev& bvh, const float* rays, size_t n, uint32_t* out, cudaStream_t st);

@@ -225,13 +225,71 @@ __global__ void __launch_bounds__(256) k_rt_push(MaskPtrs masks, CostPtrs costs,
     }
 }
 
+// spp > 1: k_rt_push for the count image (one byte per pixel): mask rows [b0, b1) are the image rows [4 * b0, min(4 * b1, H)), whose
+// byte range need not start or end on a 16-byte boundary (W is arbitrary), so the 16-byte body is framed by a byte-wise head and tail.
+struct CountPtrs { uint8_t* p[HR_MAX_RANKS]; };
+__global__ void __launch_bounds__(256) k_rt_push_count(CountPtrs counts, CostPtrs costs, int* __restrict__ ctl, uint32_t* __restrict__ acc, TickPtrs ticks, int world,
+                                                       int self, int parity, int MH, int W, int H, int tick)
+{
+    const int    b0 = ctl[self], b1 = ctl[self + 1];
+    const size_t first = (size_t)4 * b0 * W, last = (size_t)min(4 * b1, H) * W;
+    const size_t a0 = min((first + 15) & ~(size_t)15, last), a1 = max(last & ~(size_t)15, a0); // 16-byte aligned body [a0, a1)
+    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
+    const uint8_t* src = counts.p[self];
+    for (size_t i = a0 / 16 + tid; i < a1 / 16; i += nthr)
+    {
+        const uint4 v = reinterpret_cast<const uint4*>(src)[i];
+        for (int r = 0; r < world; r++)
+            if (r != self) reinterpret_cast<uint4*>(counts.p[r])[i] = v;
+    }
+    if (tid < 32)
+    {
+        const size_t i = tid < 16 ? first + tid : a1 + (tid - 16); // head: [first, a0), tail: [a1, last), 15 bytes at most each
+        if (i < (tid < 16 ? a0 : last))
+        {
+            const uint8_t v = src[i];
+            for (int r = 0; r < world; r++)
+                if (r != self) counts.p[r][i] = v;
+        }
+    }
+    // the cost drain and the tick: as in k_rt_push
+    if (blockIdx.x == 0)
+        for (int row = b0 + threadIdx.x; row < b1; row += blockDim.x)
+        {
+            const uint32_t v = acc[row];
+            acc[row]         = 0u;
+            for (int r = 0; r < world; r++) costs.p[r][(size_t)parity * MH + row] = v;
+        }
+    __threadfence_system();
+    __syncthreads();
+    __shared__ int s_last;
+    if (threadIdx.x == 0)
+    {
+        const int done = atomicAdd(ctl + HR_MAX_RANKS + 2, 1);
+        s_last         = done == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    if (threadIdx.x == 0)
+    {
+        ctl[HR_MAX_RANKS + 2] = 0; // blocks-done counter
+    }
+    const int r = threadIdx.x;
+    if (r < world && r != self && ticks.p[r])
+    {
+        __threadfence_system(); // all blocks' stores (ordered before their atomicAdd) are visible before the tick
+        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
+    }
+}
+
 // One warp.  Lanes spin until every peer's ray-trace tick reached `rt_tick` and its history tick `hist_tick` (10 s time-out),
 // then the warp computes next frame's partition: bounds[k] = first mask row whose cost prefix reaches k/world of the total.
-// Every rank computes the same table from the same (complete) cost table.
+// Every rank computes the same table from the same (complete) cost table.  Any height: each lane sums one 1/32 chunk of the
+// rows; a bound lies in the chunk of the first lane whose inclusive chunk prefix reaches its target, which the warp then scans
+// 32 rows at a time.
 __global__ void k_rt_wait_partition(const int* __restrict__ ticks, int rt_tick, int hist_tick, int* err, const uint32_t* __restrict__ cost, int MH, int world, int self,
                                     int cap, int* __restrict__ bounds)
 {
-    __shared__ unsigned long long s_prefix[1024 + 1];
     const int lane = threadIdx.x;
     if (lane < world && lane != self)
     {
@@ -259,37 +317,46 @@ __global__ void k_rt_wait_partition(const int* __restrict__ ticks, int rt_tick, 
         if (lane >= o) incl += v;
     }
     const unsigned long long total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    unsigned long long       run   = incl - local;
-    if (MH <= 1024)
+    int                      prev  = 0;
+    if (lane == 0) bounds[0] = 0;
+    for (int k = 1; k < world; k++)
     {
-        for (int i = lane * chunk; i < min((lane + 1) * chunk, MH); i++) { run += __ldcg(cost + i); s_prefix[i + 1] = run; }
-        if (lane == 0) s_prefix[0] = 0;
-    }
-    __syncwarp();
-    if (lane == 0)
-    {
-        int prev  = 0;
-        bounds[0] = 0;
-        for (int k = 1; k < world; k++)
+        int b;
+        if (total == 0) b = (int)(((long long)MH * k) / world); // no cost information: uniform split
+        else
         {
-            int b;
-            if (total == 0 || MH > 1024) b = (int)(((long long)MH * k) / world); // no cost information: uniform split
-            else
+            // first row index b with prefix[b] >= target (prefix[b] = sum of cost[0, b)), at least prev
+            const unsigned long long target = (total * (unsigned long long)k) / (unsigned long long)world;
+            int                      first  = 0;
+            if (target > 0)
             {
-                const unsigned long long target = (total * (unsigned long long)k) / (unsigned long long)world;
-                int lo = prev, hi = MH; // first row index b with prefix[b] >= target
-                while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_prefix[mid] >= target) hi = mid; else lo = mid + 1; }
-                b = lo;
+                const int          L   = __ffs(__ballot_sync(0xFFFFFFFFu, incl >= target)) - 1; // lanes past the rows hold incl == total
+                unsigned long long run = __shfl_sync(0xFFFFFFFFu, incl - local, L);
+                const int          r1  = min((L + 1) * chunk, MH);
+                for (int r0 = L * chunk;; r0 += 32) // ends inside the chunk: its inclusive prefix reaches the target
+                {
+                    const int          i = r0 + lane;
+                    unsigned long long v = i < r1 ? __ldcg(cost + i) : 0ull;
+                    for (int o = 1; o < 32; o <<= 1)
+                    {
+                        const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, v, o);
+                        if (lane >= o) v += u;
+                    }
+                    const unsigned m = __ballot_sync(0xFFFFFFFFu, i < r1 && run + v >= target);
+                    if (m) { first = r0 + __ffs(m); break; } // prefix[i + 1] reaches the target first
+                    run += __shfl_sync(0xFFFFFFFFu, v, 31);
+                }
             }
-            b = max(b, prev + 1);               // at least one row per rank
-            b = min(b, prev + cap);             // the fixed launch grid covers at most `cap` rows
-            b = min(b, MH - (world - k));       // leave a row for each remaining rank
-            b = max(b, MH - (world - k) * cap); // the remaining ranks must be able to cover the rest
-            bounds[k] = b;
-            prev      = b;
+            b = max(first, prev);
         }
-        bounds[world] = MH;
+        b = max(b, prev + 1);               // at least one row per rank
+        b = min(b, prev + cap);             // the fixed launch grid covers at most `cap` rows
+        b = min(b, MH - (world - k));       // leave a row for each remaining rank
+        b = max(b, MH - (world - k) * cap); // the remaining ranks must be able to cover the rest
+        if (lane == 0) bounds[k] = b;
+        prev = b;
     }
+    if (lane == 0) bounds[world] = MH;
 }
 
 __global__ void k_peer_wait(const int* __restrict__ ticks, int world, int self, int tick, int* err)
@@ -349,6 +416,22 @@ __global__ void __launch_bounds__(256) k_rt_push_chunks(RowPtrs imgs, NeedRows n
     }
 }
 
+// The two count images of the cooperative spp > 1 trace (shared images 7-8, by frame parity): allocated when a shadows / AO pass is
+// linked, so only linked passes pay their 2 B per pass pixel (16.6 MB at 3840x2160, 66 MB at 7680x4320).  They exist before the
+// first render, so switching spp on linked ranks needs no further collective.
+int rt_alloc_counts(hr_pass* p)
+{
+    if (p->n_hist < 9 || p->count_pp[0]) return HR_OK;
+    for (int k = 0; k < 2; k++)
+    {
+        HR_CUDA(p->ctx, cudaMalloc((void**)&p->count_pp[k], (size_t)p->W * p->H));
+        p->allocs.push_back(p->count_pp[k]);
+        HR_CUDA(p->ctx, cudaMemset(p->count_pp[k], 0, (size_t)p->W * p->H));
+        p->hist_local[7 + k] = p->count_pp[k];
+    }
+    return HR_OK;
+}
+
 int peer_alloc_ticks(hr_pass* p)
 {
     hr_ctx* ctx = p->ctx;
@@ -376,6 +459,7 @@ int hr_peer_link_ipc(hr_pass* p, cudaStream_t st)
     if (p->peers_linked || ctx->world <= 1 || !ctx->nccl_comm || p->n_hist == 0) return HR_OK;
     NcclApi& N = nccl();
     int      rc = peer_alloc_ticks(p);
+    if (rc == HR_OK) rc = rt_alloc_counts(p);
     if (rc != HR_OK) return rc;
     const int    nh = p->n_hist + 1, world = ctx->world;
     const size_t hb = sizeof(cudaIpcMemHandle_t), mine = hb * nh;
@@ -519,7 +603,7 @@ static int rt_init_bounds(hr_pass* p)
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out)
 {
     hr_ctx* ctx = p->ctx;
-    if (!p->peers_linked || ctx->world <= 1 || p->n_hist < 7) return false;
+    if (!p->peers_linked || ctx->world <= 1 || p->n_hist < 9) return false;
     RtShare sh {};
     sh.mask_local = static_cast<uint32_t*>(p->hist_local[4 + parity]);
     sh.bounds     = p->rt_bounds;
@@ -530,20 +614,24 @@ bool hr_rt_share(hr_pass* p, int parity, RtShare* out)
     return true;
 }
 
-int hr_rt_share_finish(hr_pass* p, int parity, int tick, cudaStream_t st)
+int hr_rt_share_finish(hr_pass* p, int parity, int tick, bool count, cudaStream_t st)
 {
     hr_ctx*   ctx = p->ctx;
     const int MH = (p->H + 3) / 4, MW = (p->W + 7) / 8;
     CostPtrs  c {};
     MaskPtrs  m {};
+    CountPtrs n {};
     TickPtrs  t {};
     for (int r = 0; r < ctx->world; r++)
     {
         c.p[r] = static_cast<uint32_t*>(p->hist_peer[r][6]);
         m.p[r] = static_cast<uint32_t*>(p->hist_peer[r][4 + parity]);
+        n.p[r] = static_cast<uint8_t*>(p->hist_peer[r][7 + parity]);
         t.p[r] = p->peer_ticks[r];
     }
-    k_rt_push<<<32, 256, 0, st>>>(m, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, MW, tick);
+    // a count row holds 8x the bytes of a mask row: more blocks for the wider copy
+    if (count) k_rt_push_count<<<128, 256, 0, st>>>(n, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, p->W, p->H, tick);
+    else k_rt_push<<<32, 256, 0, st>>>(m, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, MW, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -607,8 +695,9 @@ int hr_shard_link_local(hr_pass* pass, int rank, hr_pass* peer)
                         pass->W == peer->W && pass->H == peer->H && !pass->peers_ipc,
                HR_ERR_INVALID_ARG, "hr_shard_link_local: passes do not match (kind / size / rank) or the pass has no peer history");
     int rc = peer_alloc_ticks(pass);
-    if (rc != HR_OK) return rc;
-    rc = peer_alloc_ticks(peer);
+    if (rc == HR_OK) rc = peer_alloc_ticks(peer);
+    if (rc == HR_OK) rc = rt_alloc_counts(pass);
+    if (rc == HR_OK) rc = rt_alloc_counts(peer);
     if (rc != HR_OK) return rc;
     for (int k = 0; k < pass->n_hist; k++) pass->hist_peer[rank][k] = peer->hist_local[k];
     pass->peer_ticks[rank] = peer->sync_ticks;

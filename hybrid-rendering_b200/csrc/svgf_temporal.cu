@@ -326,11 +326,12 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
 // ---- spp > 1: count image instead of the bit mask (SURVEY.md §8d; not in the reference) ---------------------------------
 // Same kernel as k_temporal<MODE, false> except for where the visibility comes from: the 17x17 box mean is the sum of an
 // 8-bit count tile (separable: 17-wide row sums, then 17 rows) divided by 289 * spp, the pixel's visibility is count / spp.
-// Kept as a separate kernel so the 1-spp path stays exactly what the parity runs validated.  Single GPU only.
-template <int MODE>
-__global__ void __launch_bounds__(256, 4) k_temporal_count(GBufLevelDev cur, GBufLevelDev prev, const uint8_t* __restrict__ count, int spp, const HistPeers hp,
-                                                   FrameConsts fc, float alpha_p, float moments_alpha_p,
-                                                   void* __restrict__ out_img, void* __restrict__ out_aux, uint8_t* __restrict__ tile_flags, int row0, int row1)
+// Kept as a separate kernel so the 1-spp path stays exactly what the parity runs validated.  PEER: linked ranks read a history texel
+// from the rank that owns its row (hist_ld32 / hist_ld16), like k_temporal<MODE, true>.
+template <int MODE, bool PEER>
+__device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev prev, const uint8_t* __restrict__ count, int spp, const HistPeers hp, FrameConsts fc,
+                                               float alpha_p, float moments_alpha_p, void* __restrict__ out_img, void* __restrict__ out_aux,
+                                               uint8_t* __restrict__ tile_flags, int row0, int row1)
 {
     __shared__ unsigned char  s_cnt[24][48]; // unoccluded rays per pixel, region rows y0-8 .. y0+15, columns x0-8 .. x0+39
     __shared__ unsigned short s_h[24][34];   // per-row 17-wide sums
@@ -407,8 +408,8 @@ __global__ void __launch_bounds__(256, 4) k_temporal_count(GBufLevelDev cur, GBu
                 const float w4[4] = { (1 - fx) * (1 - fy), fx * (1 - fy), (1 - fx) * fy, fx * fy };
                 {
                     const size_t hi = (size_t)hcy * W + hcx;
-                    if (MODE == 0) hist_len = h2_to_f2(hist_ld32<false>(hp.aux, hp, hcy, 2 * hi + 1)).x;
-                    else hist_len = __half2float(__ushort_as_half((unsigned short)hist_ld16<false>(hp.aux, hp, hcy, hi)));
+                    if (MODE == 0) hist_len = h2_to_f2(hist_ld32<PEER>(hp.aux, hp, hcy, 2 * hi + 1)).x;
+                    else hist_len = __half2float(__ushort_as_half((unsigned short)hist_ld16<PEER>(hp.aux, hp, hcy, hi)));
                 }
                 TapRaw   tr[4];
                 uint32_t hraw[4], mraw[4];
@@ -428,10 +429,10 @@ __global__ void __launch_bounds__(256, 4) k_temporal_count(GBufLevelDev cur, GBu
                         tr[s] = fetch_prev_raw(prev, pi);
                         if (MODE == 0)
                         {
-                            hraw[s] = hist_ld32<false>(hp.img, hp, py, pi);
-                            mraw[s] = hist_ld32<false>(hp.aux, hp, py, 2 * pi);
+                            hraw[s] = hist_ld32<PEER>(hp.img, hp, py, pi);
+                            mraw[s] = hist_ld32<PEER>(hp.aux, hp, py, 2 * pi);
                         }
-                        else hraw[s] = hist_ld16<false>(hp.img, hp, py, pi);
+                        else hraw[s] = hist_ld16<PEER>(hp.img, hp, py, pi);
                     }
                 }
                 const float3 cn   = octohedral_to_direction(g2.x, g2.y);
@@ -473,12 +474,12 @@ __global__ void __launch_bounds__(256, 4) k_temporal_count(GBufLevelDev cur, GBu
                                     const size_t pi = (size_t)py * W + px;
                                     if (MODE == 0)
                                     {
-                                        hcol += h2_to_f2(hist_ld32<false>(hp.img, hp, py, pi)).x;
-                                        const float2 mm = h2_to_f2(hist_ld32<false>(hp.aux, hp, py, 2 * pi));
+                                        hcol += h2_to_f2(hist_ld32<PEER>(hp.img, hp, py, pi)).x;
+                                        const float2 mm = h2_to_f2(hist_ld32<PEER>(hp.aux, hp, py, 2 * pi));
                                         hm0 += mm.x;
                                         hm1 += mm.y;
                                     }
-                                    else hcol += __half2float(__ushort_as_half((unsigned short)hist_ld16<false>(hp.img, hp, py, pi)));
+                                    else hcol += __half2float(__ushort_as_half((unsigned short)hist_ld16<PEER>(hp.img, hp, py, pi)));
                                 }
                                 cntv += 1.0f;
                             }
@@ -538,6 +539,21 @@ __global__ void __launch_bounds__(256, 4) k_temporal_count(GBufLevelDev cur, GBu
     }
 }
 
+#define TEMPORAL_COUNT_PARAMS                                                                                                           \
+    GBufLevelDev cur, GBufLevelDev prev, const uint8_t* __restrict__ count, int spp, const HistPeers hp, FrameConsts fc, float alpha_p, \
+        float moments_alpha_p, void* __restrict__ out_img, void* __restrict__ out_aux, uint8_t* __restrict__ tile_flags, int row0, int row1
+template <int MODE>
+__global__ void __launch_bounds__(256, 4) k_temporal_count(TEMPORAL_COUNT_PARAMS)
+{
+    temporal_count<MODE, false>(cur, prev, count, spp, hp, fc, alpha_p, moments_alpha_p, out_img, out_aux, tile_flags, row0, row1);
+}
+template <int MODE>
+__global__ void __launch_bounds__(256, 4) k_temporal_count_peer(TEMPORAL_COUNT_PARAMS)
+{
+    temporal_count<MODE, true>(cur, prev, count, spp, hp, fc, alpha_p, moments_alpha_p, out_img, out_aux, tile_flags, row0, row1);
+}
+#undef TEMPORAL_COUNT_PARAMS
+
 } // namespace
 
 void launch_shadows_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint32_t* mask, const HistPeers& hist, const FrameConsts& fc, float alpha,
@@ -563,7 +579,8 @@ void launch_shadows_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& 
 {
     if (row1 <= row0) return;
     dim3 grid((cur.W + 31) / 32, (row1 - row0 + 7) / 8);
-    k_temporal_count<0><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, moments_alpha, out, moments_out, tile_flags, row0, row1);
+    if (hist.world > 1) k_temporal_count_peer<0><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, moments_alpha, out, moments_out, tile_flags, row0, row1);
+    else k_temporal_count<0><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, moments_alpha, out, moments_out, tile_flags, row0, row1);
 }
 
 void launch_ao_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
@@ -571,5 +588,6 @@ void launch_ao_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev,
 {
     if (row1 <= row0) return;
     dim3 grid((cur.W + 31) / 32, (row1 - row0 + 7) / 8);
-    k_temporal_count<1><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, 0.0f, out, len_out, tile_flags, row0, row1);
+    if (hist.world > 1) k_temporal_count_peer<1><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, 0.0f, out, len_out, tile_flags, row0, row1);
+    else k_temporal_count<1><<<grid, 256, 0, st>>>(cur, prev, count, spp, hist, fc, alpha, 0.0f, out, len_out, tile_flags, row0, row1);
 }

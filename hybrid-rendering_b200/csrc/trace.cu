@@ -176,6 +176,30 @@ __global__ void __launch_bounds__(RT_CTA_WARPS * 32) k_ray_trace_mask_shared(GBu
     count_rays(fc.ray_ctr, 0, traced ? 1u : 0u);
 }
 
+// spp > 1 form of the cooperative trace: the share's pixels go to this rank's count image (k_rt_push_count copies them to the
+// peers).  trace_pixel_spp is the function of k_ray_trace_count, so the counts equal the single-GPU counts bit for bit.  A warp's
+// duration grows about linearly with spp, so it is added to the row cost in units of 2^cost_shift cycles, cost_shift = 6 +
+// ceil(log2 spp): the row sums stay in the range of the 1-spp trace (scaling every row alike leaves the partition unchanged)
+// and cannot overflow at spp <= 255.
+template <int MODE>
+__global__ void __launch_bounds__(RT_CTA_WARPS * 32) k_ray_trace_count_shared(GBufLevelDev g, BvhDev bvh, FrameConsts fc, float p0, float p1, const uint8_t* __restrict__ sobol,
+                                                                                 const uint8_t* __restrict__ sr, uint8_t* __restrict__ count, int spp, int cost_shift, RtShare sh)
+{
+    const long long t0 = clock64();
+    const int MW   = (g.W + 7) >> 3;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int mrow0 = __ldg(sh.bounds + sh.self), mrow1 = __ldg(sh.bounds + sh.self + 1);
+    const int mx = blockIdx.x * RT_CTA_WARPS + warp, my = mrow0 + blockIdx.y;
+    if (mx >= MW || my >= mrow1) return; // whole warp exits together
+    const int      x = mx * 8 + (lane & 7), y = my * 4 + (lane >> 3);
+    uint32_t       n_traced;
+    const uint32_t n = trace_pixel_spp<MODE>(g, bvh, fc, p0, p1, sobol, sr, x, y, spp, n_traced);
+    if (x < g.W && y < g.H) count[(size_t)y * g.W + x] = (uint8_t)n;
+    __syncwarp();
+    if (lane == 0) atomicAdd(sh.cost_acc + my, (uint32_t)((clock64() - t0) >> cost_shift) + 1u);
+    count_rays(fc.ray_ctr, 0, n_traced);
+}
+
 __global__ void k_trace_any(BvhDev bvh, const float* __restrict__ rays, size_t n, uint32_t* __restrict__ out)
 {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -225,6 +249,16 @@ void launch_ray_trace_mask_shared(int kind, const GBufLevelDev& g, const BvhDev&
     const dim3 grid(((g.W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, hr_rt_share_cap((g.H + 3) / 4, sh.world), 1);
     const auto k = kind == PASS_AO ? k_ray_trace_mask_shared<1> : k_ray_trace_mask_shared<0>;
     k<<<grid, RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, sobol, sr, sh);
+}
+
+void launch_ray_trace_count_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
+                                   const uint8_t* sr, uint8_t* count, int spp, const RtShare& sh, cudaStream_t st)
+{
+    int cost_shift = 6;
+    while ((1 << (cost_shift - 6)) < spp) cost_shift++;
+    const dim3 grid(((g.W + 7) / 8 + RT_CTA_WARPS - 1) / RT_CTA_WARPS, hr_rt_share_cap((g.H + 3) / 4, sh.world), 1);
+    const auto k = kind == PASS_AO ? k_ray_trace_count_shared<1> : k_ray_trace_count_shared<0>;
+    k<<<grid, RT_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, sobol, sr, count, spp, cost_shift, sh);
 }
 
 void launch_ray_trace_count(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,

@@ -272,8 +272,12 @@ typedef struct hr_shadows_params { /* defaults: src/ray_traced_shadows.h:50-115 
     int32_t denoise;            /* 1    */
     int32_t spp;                /* 1: the reference's single ray per pixel.  > 1 (SURVEY.md §8d configs 4-5, not in the reference):
                                  * spp rays per pixel, sample index num_frames * spp + s; output 0 becomes an R8_UINT W x H image
-                                 * of unoccluded-ray counts, the temporal stage uses visibility = count / spp; single GPU only;
-                                 * 0 is read as 1 */
+                                 * of unoccluded-ray counts, the temporal stage uses visibility = count / spp.  Linked ranks
+                                 * (hr_shard_init, or hr_shard_config + hr_shard_link_local) trace the count image cooperatively
+                                 * like the 1-spp mask: each traces a cost-balanced share of the rows and pushes it to every peer,
+                                 * so output 0 is complete on every rank; results are bit-identical to one GPU.  A linked shadows /
+                                 * AO pass holds two W x H count images from link time (2 B per pass pixel: 16.6 MB at 3840 x 2160);
+                                 * 0 is read as 1; at most 255 */
 } hr_shadows_params;
 
 /* OutputType, src/ray_traced_shadows.h:10-16 (+ internals for tests) */
@@ -302,7 +306,7 @@ typedef struct hr_ao_params { /* defaults: src/ray_traced_ao.h:51-110 */
     float   power;       /* 1.2  */
     int32_t blur_radius; /* 4    */
     int32_t denoise;     /* 1    */
-    int32_t spp;         /* 1; > 1: see hr_shadows_params.spp */
+    int32_t spp;         /* 1; > 1: see hr_shadows_params.spp (count image, cooperative trace on linked ranks) */
 } hr_ao_params;
 
 enum {
@@ -404,7 +408,8 @@ typedef struct hr_reflections_params { /* defaults: src/ray_traced_reflections.h
     float   sky_color[3];          /* miss colour (skybox cubemap replaced by a constant) */
     int32_t spp;                   /* 1: the reference's single ray per pixel.  > 1 (SURVEY.md §8d configs 4-5, not in the reference): the GGX
                                     * lobe draws spp directions (sample index num_frames * spp + s) and stores the mean of the clamped
-                                    * radiance; the ray length is the first sample's; 0 is read as 1 */
+                                    * radiance; the ray length is the first sample's; 0 is read as 1.  Linked ranks trace the
+                                    * interleaved 8-row chunks at every spp (DESIGN.md §9), bit-identical to one GPU */
 } hr_reflections_params;
 
 enum {
