@@ -71,15 +71,16 @@ __device__ __forceinline__ V3 world_position_from_depth(float u, float v, float 
 }
 
 // bnd_sampler.glsl:4-24 on raw bytes
-__device__ __forceinline__ float sample_blue_noise(int x, int y, int sample_index, int dim, const uint8_t* __restrict__ sobol,
+// sample_index: num_frames * spp + s in uint32 arithmetic (DESIGN.md §7), defined for every hr_frame::num_frames
+__device__ __forceinline__ float sample_blue_noise(int x, int y, uint32_t sample_index, int dim, const uint8_t* __restrict__ sobol,
                                                    const uint8_t* __restrict__ sr)
 {
     x &= 127;
     y &= 127;
-    sample_index &= 255;
+    sample_index &= 255u;
     dim &= 3;
     const uint8_t* t     = sr + 4 * (y * 128 + x);
-    const int      rsi   = sample_index ^ (int)t[2];
+    const int      rsi   = (int)sample_index ^ (int)t[2];
     int            value = (int)sobol[4 * rsi + dim];
     value ^= (int)t[dim & 1];
     return (0.5f + (float)value) / 256.0f;

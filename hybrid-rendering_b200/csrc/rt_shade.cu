@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
         }
         else
         {
-            const int   si = (int)fc.num_frames * spp + s;
+            const uint32_t si = fc.num_frames * (uint32_t)spp + (uint32_t)s;
             const float ex = det::sample_blue_noise(x, y, si, 0, sobol, srk) * P.trim;
             const float ey = det::sample_blue_noise(x, y, si, 1, sobol, srk) * P.trim;
             const V3    Wh = importance_sample_ggx(ex, ey, N, roughness);

@@ -281,6 +281,8 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
                 int cnt = 0;
 #pragma unroll
                 for (int r = 0; r < 17; r++) cnt += s_h[ly + r][lx];
+                // a multiply by the rounded 1/289 is enough here (unlike temporal_count): visibility is 0 or 1, and cnt * (1/289)
+                // is exactly 1 for an all-open window (cnt = 289) and exactly 0 for a closed one, so no tile flag can move
                 const float mean = (float)cnt * (1.0f / 289.0f);
                 const float sd   = sqrtf(fmaxf(mean - mean * mean, 0.0f));
                 hcol             = fminf(fmaxf(hcol, mean - 0.5f * sd), mean + 0.5f * sd);
@@ -386,7 +388,10 @@ __device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev pr
         if (MODE == 1) o0 = 1.0f;
         if (depth != 1.0f)
         {
-            const float vis = (float)s_cnt[ly + 8][lx + 8] * (1.0f / (float)spp);
+            // count / spp and the box mean below are exact quotients, as the oracle computes them: a multiply by the rounded
+            // reciprocal gives 0.99999994 for count == spp at spp 41, 47, 55, ... and an all-open window's mean one ulp off 1 at
+            // spp 3, 6, 7, ..., which flips `o0 < 1` / `o0 > 0` tile flags.  Both quotients are exact: 289 * 255 < 2^24.
+            const float vis = __fdiv_rn((float)s_cnt[ly + 8][lx + 8], (float)spp);
             // ---- reproject(), reprojection.glsl:115-328 ----
             const float  fw = (float)W, fh = (float)H;
             const float  tu = ((float)x + 0.5f) * fast_rcp(fw), tv = ((float)y + 0.5f) * fast_rcp(fh);
@@ -497,7 +502,7 @@ __device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev pr
                 int cnt = 0;
 #pragma unroll
                 for (int r = 0; r < 17; r++) cnt += s_h[ly + r][lx];
-                const float mean = (float)cnt * (1.0f / (289.0f * (float)spp));
+                const float mean = __fdiv_rn((float)cnt, 289.0f * (float)spp);
                 const float sd   = sqrtf(fmaxf(mean - mean * mean, 0.0f));
                 hcol             = fminf(fmaxf(hcol, mean - 0.5f * sd), mean + 0.5f * sd);
             }

@@ -41,8 +41,8 @@ __device__ __forceinline__ uint32_t trace_pixel(const GBufLevelDev& g, const Bvh
             const V3     P  = det::world_position_from_depth(u, v, depth, fc.view_proj_inverse);
             const float2 e  = load_oct_normal(g.gb2, idx);
             const V3     N  = det::octohedral_to_direction(e.x, e.y);
-            const float  r0 = det::sample_blue_noise(x, y, (int)fc.num_frames, 0, sobol, sr);
-            const float  r1 = det::sample_blue_noise(x, y, (int)fc.num_frames, 1, sobol, sr);
+            const float  r0 = det::sample_blue_noise(x, y, fc.num_frames, 0, sobol, sr);
+            const float  r1 = det::sample_blue_noise(x, y, fc.num_frames, 1, sobol, sr);
             Ray          r;
             r.tmin = 0.01f;
             if (MODE == 0)
@@ -105,7 +105,7 @@ __device__ __forceinline__ uint32_t trace_pixel_spp(const GBufLevelDev& g, const
             const V3     N  = det::octohedral_to_direction(e.x, e.y);
             for (int s = 0; s < spp; s++)
             {
-                const int   si = (int)fc.num_frames * spp + s;
+                const uint32_t si = fc.num_frames * (uint32_t)spp + (uint32_t)s;
                 const float r0 = det::sample_blue_noise(x, y, si, 0, sobol, sr);
                 const float r1 = det::sample_blue_noise(x, y, si, 1, sobol, sr);
                 Ray         r;

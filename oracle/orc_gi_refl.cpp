@@ -243,7 +243,7 @@ void reflections_ray_trace(const ShadingScene& ss, const GBufLevel& g, const hr_
             }
             else
             {
-                const int si = (int)f.num_frames * spp + smp;
+                const uint32_t si = f.num_frames * (uint32_t)spp + (uint32_t)smp;
                 vec2 Xi = { sample_blue_noise(c, si, 0, bn) * rp.trim, sample_blue_noise(c, si, 1, bn) * rp.trim };
                 vec3 Wh = importance_sample_ggx(Xi, N, roughness);
                 dir     = reflect(-Wo, Wh);

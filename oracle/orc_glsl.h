@@ -106,14 +106,16 @@ struct BlueNoise {
     const uint8_t* sobol;     // 256 x RGBA8
     const uint8_t* scr_rank;  // 128 x 128 x RGBA8
 };
-inline float sample_blue_noise(ivec2 coord, int sample_index, int sample_dimension, const BlueNoise& bn)
+// sample_index is unsigned (DESIGN.md §7): callers pass num_frames * spp + s in uint32 arithmetic, so every hr_frame::num_frames
+// maps to (num_frames * spp + s) mod 256.  The shader's `% 256` on a signed int would be negative for indices >= 2^31.
+inline float sample_blue_noise(ivec2 coord, uint32_t sample_index, int sample_dimension, const BlueNoise& bn)
 {
     coord.x          = coord.x % 128;
     coord.y          = coord.y % 128;
-    sample_index     = sample_index % 256;
+    sample_index     = sample_index & 255u;
     sample_dimension = sample_dimension % 4;
     const uint8_t* sr = bn.scr_rank + 4 * (coord.y * 128 + coord.x);
-    int ranked_sample_index = sample_index ^ (int)sr[2];
+    int ranked_sample_index = (int)sample_index ^ (int)sr[2];
     int value               = (int)bn.sobol[4 * ranked_sample_index + sample_dimension];
     value                   = value ^ (int)sr[sample_dimension % 2];
     return (0.5f + (float)value) / 256.0f;

@@ -46,7 +46,7 @@ void shadows_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f
                     vec4 gb2        = g.fetch2(c);
                     vec3 normal     = octohedral_to_direction({ gb2.x, gb2.y });
                     vec3 ray_origin = world_pos + normal * bias;
-                    vec2 rnd        = { sample_blue_noise(c, (int)f.num_frames, 0, bn), sample_blue_noise(c, (int)f.num_frames, 1, bn) };
+                    vec2 rnd        = { sample_blue_noise(c, f.num_frames, 0, bn), sample_blue_noise(c, f.num_frames, 1, bn) };
                     vec3  Wi;
                     float t_max, attenuation;
                     fetch_light_properties_shadow(f.ubo.light, world_pos, normal, rnd, Wi, t_max, attenuation);
@@ -81,7 +81,7 @@ void ao_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f, flo
                     vec4 gb2        = g.fetch2(c);
                     vec3 normal     = octohedral_to_direction({ gb2.x, gb2.y });
                     vec3 ray_origin = world_pos + normal * bias;
-                    vec2 rnd        = { sample_blue_noise(c, (int)f.num_frames, 0, bn), sample_blue_noise(c, (int)f.num_frames, 1, bn) };
+                    vec2 rnd        = { sample_blue_noise(c, f.num_frames, 0, bn), sample_blue_noise(c, f.num_frames, 1, bn) };
                     vec3 dir        = sample_cosine_lobe(normal, rnd);
                     result          = (uint32_t)scene.query_visibility(ray_origin, dir, ray_length);
                 }
@@ -115,7 +115,7 @@ void ray_trace_count(const Scene& scene, const GBufLevel& g, const hr_frame& f, 
                 const vec3 ray_origin = world_pos + normal * bias;
                 for (int s = 0; s < spp; s++)
                 {
-                    const int  idx = (int)f.num_frames * spp + s;
+                    const uint32_t idx = f.num_frames * (uint32_t)spp + (uint32_t)s;
                     const vec2 rnd = { sample_blue_noise(c, idx, 0, bn), sample_blue_noise(c, idx, 1, bn) };
                     if (ao) n += (uint32_t)scene.query_visibility(ray_origin, sample_cosine_lobe(normal, rnd), p0);
                     else
@@ -517,7 +517,7 @@ void orc_trace_closest(void* sp, const float* rays, size_t n, float* out_t, uint
 
 void orc_det_sincos(const float* x, size_t n, float* s, float* c) { for (size_t i = 0; i < n; i++) det_sincos(x[i], s + i, c + i); }
 void orc_oct_decode(const float* e, size_t n, float* out) { for (size_t i = 0; i < n; i++) { vec3 v = octohedral_to_direction({ e[2*i], e[2*i+1] }); out[3*i]=v.x; out[3*i+1]=v.y; out[3*i+2]=v.z; } }
-float orc_sample_blue_noise(int x, int y, int idx, int dim, const uint8_t* sobol, const uint8_t* sr) { BlueNoise bn{ sobol, sr }; return sample_blue_noise({ x, y }, idx, dim, bn); }
+float orc_sample_blue_noise(int x, int y, int idx, int dim, const uint8_t* sobol, const uint8_t* sr) { BlueNoise bn{ sobol, sr }; return sample_blue_noise({ x, y }, (uint32_t)idx, dim, bn); }
 
 void orc_build_mip(int W, int H, const uint16_t* gb2, const uint16_t* gb3, const float* depth, uint16_t* ogb2, uint16_t* ogb3, float* odepth)
 { build_mip(W, H, gb2, gb3, depth, ogb2, ogb3, odepth); }

@@ -325,23 +325,20 @@ def test_reflections_phi_normal_ragged():
 
 
 # ---------------------------------------------------------------------------------------------- full-resolution post chain
-@pytest.mark.parametrize("W,H", [(250, 141), (251, 144)])
-def test_post_chain_ragged(W, H):
-    """deferred combine over the device's own pass outputs, TAA over it (bit-exact), tone map, and the path tracer"""
-    sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
-    ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
-    ctx = new_context(sc, W, H)
+def run_post_chain(case, ctx, W, H, seq):
+    """deferred combine over the device's own pass outputs, TAA over it (bit-exact, jittered by the frame's num_frames) and tone map,
+    over the (i, frame) sequence `seq`"""
     sh, ao, rf, de = pyhr.Pass(ctx, "shadows", W, H, 0), pyhr.Pass(ctx, "ao", W, H, 1), pyhr.ReflectionsPass(ctx, W, H, 1), pyhr.DeferredPass(ctx, W, H)
     rf.params.sky_color[0], rf.params.sky_color[1], rf.params.sky_color[2] = SKY
     de.params.env_color[0], de.params.env_color[1], de.params.env_color[2] = SKY
     taa, tm = pyhr.TAAPass(ctx, W, H), pyhr.TonemapPass(ctx, W, H)
     taa.params.reset_every_frame = 0  # the history feeds the next frame
     otaa = O.TAAOracle(W, H, reset_every_frame=0)
-    w = Worst(f"post chain {W}x{H}")
+    w = Worst(case)
     prev_j = np.zeros(2, np.float32)
-    for i, f in frames(W, H, 5, pan_from=2):
-        j = pyhr.taa_jitter(i, W, H)
-        assert np.array_equal(j, O.taa_jitter(i, W, H))
+    for i, f in seq:
+        j = pyhr.taa_jitter(f.num_frames, W, H)
+        assert np.array_equal(j, O.taa_jitter(f.num_frames, W, H))
         pyhr.apply_jitter(f, j, prev_j)
         prev_j = j
         ctx.gbuffer_render(f.ping_pong, f)
@@ -372,6 +369,17 @@ def test_post_chain_ragged(W, H):
         d = np.abs(got8.astype(np.int16) - want8.astype(np.int16))
         assert got8.shape == (H, W, 4) and d.max() <= 1 and np.mean(d == 0) >= 0.995, f"frame {i}: tone map max diff {d.max()}, identical {np.mean(d == 0):.4f}"
     w.report()
+    for p in (tm, taa, de, rf, sh, ao):
+        p.destroy()
+
+
+@pytest.mark.parametrize("W,H", [(250, 141), (251, 144)])
+def test_post_chain_ragged(W, H):
+    """the post chain of run_post_chain, and the path tracer"""
+    sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
+    ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
+    ctx = new_context(sc, W, H)
+    run_post_chain(f"post chain {W}x{H}", ctx, W, H, frames(W, H, 5, pan_from=2))
     pt = pyhr.PathTracerPass(ctx, W, H)
     pt.params.sky_color[0], pt.params.sky_color[1], pt.params.sky_color[2] = SKY
     opt = O.PathTracerOracle(W, H, sky=SKY)
@@ -381,8 +389,7 @@ def test_post_chain_ragged(W, H):
         want = opt.render(ss, f)
         assert np.array_equal(pt.download(1), opt.prim), f"sample {i}: primary hits differ in {np.count_nonzero(pt.download(1) != opt.prim)} pixels"
         compare_path_traced(f16(pt.download(100)), f16(want), f"{W}x{H} sample {i}")
-    for p in (pt, tm, taa, de, rf, sh, ao):
-        p.destroy()
+    pt.destroy()
     ctx.close()
 
 
