@@ -1316,6 +1316,8 @@ int hr_pass_destroy(hr_pass* p)
     hr_peer_unlink(p);
     for (void* a : p->allocs) cudaFree(a);
     for (void* a : p->ddgi_grid_allocs) cudaFree(a);
+    for (void* a : p->ddgi_retired) cudaFree(a);
+    if (p->ddgi_pool) cudaMemPoolDestroy(p->ddgi_pool);
     if (p->ev_ready) cudaEventDestroy(p->ev_ready);
     if (p->ev_done) cudaEventDestroy(p->ev_done);
     for (auto& r : p->timer.recs) for (auto e : r.ev) cudaEventDestroy(e);

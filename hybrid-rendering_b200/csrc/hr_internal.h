@@ -222,6 +222,16 @@ struct hr_pass {
     uint32_t  pt_frame_idx = 0;                        // GroundTruthPathTracer::m_frame_idx
     int       pt_ping_pong = 0;                        // GroundTruthPathTracer::m_ping_pong
     std::vector<void*> ddgi_grid_allocs;
+    // linked DDGI (shard.cu): the peers' atlas addresses as this rank sees them ([rank][irradiance 0, 1, depth 0, 1], shared image 0), the
+    // frame tick of the render that published this rank's current atlases (0: not yet), the IPC mappings of the peers' atlases, the replaced
+    // atlases of an IPC rank until the next handle exchange (the peers map them), and the pool same-process ranks allocate their grids from
+    // in stream order (ddgi_grid_pooled: the current grid came from it)
+    void**    ddgi_tab = nullptr;
+    int       ddgi_ready = 0;
+    void*     ddgi_mapped[HR_MAX_RANKS][4] = {};
+    std::vector<void*> ddgi_retired;
+    cudaMemPool_t ddgi_pool = nullptr;
+    bool      ddgi_grid_pooled = false;
     // asynchronous band exchange (shard.cu): ev_ready = pass kernels done on the caller's stream, ev_done = exchange done on
     // ctx->comm_stream.  Whoever next touches an exchanged image (next frame's temporal stage, hr_pass_output/download)
     // first makes its stream wait on ev_done (hr_wait_exchange).
@@ -296,6 +306,12 @@ int  hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cu
 // WHOLE image into its own image and copies every chunk to the ranks whose denoise stages read it (rows [need0[q], need1[q]));
 // the last block publishes the ray-trace tick.
 int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* need1, cudaStream_t st); // img: the shared image (hr_peer_register index)
+// DDGI atlases of linked ranks (shard.cu): after a grid (re)initialisation, make this rank's atlas addresses known to its peers (IPC ranks:
+// a collective that maps the peers' new atlases, then frees the replaced atlases); after K19/K20, store bytes [i0, i1) of the irradiance and
+// [d0, d1) of the depth atlas of ping-pong mp into every peer's atlas and publish the atlas tick `tick` (hr_peer_wait slot 0).
+int  hr_ddgi_publish(hr_pass* p, int tick, cudaStream_t st);
+int  hr_ddgi_push(hr_pass* p, int mp, size_t i0, size_t i1, size_t d0, size_t d1, int tick, cudaStream_t st);
+void hr_ddgi_unmap(hr_pass* p); // close the IPC mappings of the peers' atlases
 // Rows of an image of height H owned by this context's rank (all rows when world == 1).
 void hr_band(const hr_ctx* ctx, int H, int* b0, int* b1);
 // [b0 - halo, b1 + halo) clamped to [0, H); halo must be a multiple of 8 so tile alignment is kept.
@@ -307,10 +323,6 @@ inline void hr_extend(int b0, int b1, int halo, int H, int* e0, int* e1)
 // Make every rank's copy of each image complete: rank r broadcasts its band of every item (one NCCL group).
 // Asynchronous: enqueued on ctx->comm_stream after everything already enqueued on `st`; completion is p->ev_done.
 int hr_shard_exchange(hr_pass* p, const ExchangeItem* items, int n, cudaStream_t st);
-// Same, with explicit per-rank row ranges [row0[r], row1[r]) (rank r broadcasts its rows of every item): DDGI atlases split by
-// probe z-slices.  SYNCHRONOUS with respect to `st`: the exchange is enqueued on `st` itself.
-struct RowRangeItem { void* base; size_t row_bytes; };
-int hr_shard_exchange_rows(hr_pass* p, const RowRangeItem* items, int n, const int* row0, const int* row1, cudaStream_t st);
 // Make `st` wait for the pass's pending exchange (no-op when nothing is pending).
 void hr_wait_exchange(hr_pass* p, cudaStream_t st);
 

@@ -15,7 +15,10 @@
 //     is >= N.  History images are double buffered by frame parity, so that wait also covers the write-after-read hazard.
 //   * the pass's FINAL OUTPUT (optional, hr_shard_set_gather; on by default): one NCCL group of point-to-point transfers (an
 //     all-gather with unequal counts: 2160 rows = 270 tiles do not divide evenly by 8) on a side stream, so every rank
-//     ends up with the complete denoised frame.  DDGI exchanges its updated probe rows with per-band broadcasts.
+//     ends up with the complete denoised frame.
+//   * DDGI ATLASES: linked ranks split the probe stages by z-slices and store their slices' atlas rows into every peer's atlas
+//     (k_ddgi_push), ordered by one frame tick; the atlases move on a grid re-initialisation, so the peers' addresses are read from
+//     a device-side table at run time.
 // The 1/2/4/8-GPU results are bit-identical to the single-GPU result (tests/test_gpu_multi.py).
 //
 // NCCL is dlopen'ed on first use so the single-GPU library has no NCCL dependency; inside a PyTorch process the
@@ -34,7 +37,6 @@ struct NcclApi {
     ncclResult_t (*CommDestroy)(ncclComm_t)                                                                    = nullptr;
     ncclResult_t (*GroupStart)()                                                                               = nullptr;
     ncclResult_t (*GroupEnd)()                                                                                 = nullptr;
-    ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)       = nullptr;
     ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t)            = nullptr;
     ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                   = nullptr; // NCCL 2.7+
     ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t)                         = nullptr; // NCCL 2.7+
@@ -59,13 +61,12 @@ NcclApi& nccl()
     LOAD(CommDestroy, "ncclCommDestroy");
     LOAD(GroupStart, "ncclGroupStart");
     LOAD(GroupEnd, "ncclGroupEnd");
-    LOAD(Broadcast, "ncclBroadcast");
     LOAD(AllGather, "ncclAllGather");
     LOAD(Send, "ncclSend");
     LOAD(Recv, "ncclRecv");
     LOAD(GetErrorString, "ncclGetErrorString");
 #undef LOAD
-    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.GroupStart && api.GroupEnd && api.Broadcast && api.AllGather && api.Send && api.Recv &&
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.GroupStart && api.GroupEnd && api.AllGather && api.Send && api.Recv &&
              api.GetErrorString;
     return api;
 }
@@ -132,23 +133,6 @@ int hr_shard_exchange(hr_pass* p, const ExchangeItem* items, int n, cudaStream_t
     return HR_OK;
 }
 
-
-int hr_shard_exchange_rows(hr_pass* p, const RowRangeItem* items, int n, const int* row0, const int* row1, cudaStream_t st)
-{
-    hr_ctx* ctx = p->ctx;
-    if (ctx->world <= 1 || !ctx->nccl_comm) return HR_OK;
-    NcclApi& N = nccl();
-    HR_NCCL(ctx, N.GroupStart());
-    for (int i = 0; i < n; i++)
-        for (int r = 0; r < ctx->world; r++)
-        {
-            if (row1[r] <= row0[r]) continue;
-            char* ptr = static_cast<char*>(items[i].base) + (size_t)row0[r] * items[i].row_bytes;
-            HR_NCCL(ctx, N.Broadcast(ptr, ptr, (size_t)(row1[r] - row0[r]) * items[i].row_bytes, ncclUint8, r, (ncclComm_t)ctx->nccl_comm, st));
-        }
-    HR_NCCL(ctx, N.GroupEnd());
-    return HR_OK;
-}
 
 // ---- peer history -----------------------------------------------------------------------------------------------------
 static int rt_init_bounds(hr_pass* p);
@@ -228,30 +212,37 @@ __global__ void __launch_bounds__(256) k_rt_push(MaskPtrs masks, CostPtrs costs,
 // spp > 1: k_rt_push for the count image (one byte per pixel): mask rows [b0, b1) are the image rows [4 * b0, min(4 * b1, H)), whose
 // byte range need not start or end on a 16-byte boundary (W is arbitrary), so the 16-byte body is framed by a byte-wise head and tail.
 struct CountPtrs { uint8_t* p[HR_MAX_RANKS]; };
-__global__ void __launch_bounds__(256) k_rt_push_count(CountPtrs counts, CostPtrs costs, int* __restrict__ ctl, uint32_t* __restrict__ acc, TickPtrs ticks, int world,
-                                                       int self, int parity, int MH, int W, int H, int tick)
+
+// Bytes [first, last) of `src` to the same offsets of every peer's image dst.p[r] (r != self; null: skipped).  The images are 256-byte
+// aligned, so a 16-byte body [a0, a1) is framed by a byte-wise head and tail of at most 15 bytes each, copied by threads 0-31 of the grid.
+template <class Ptrs>
+__device__ __forceinline__ void push_bytes(const uint8_t* __restrict__ src, const Ptrs& dst, int world, int self, size_t first, size_t last, size_t tid, size_t nthr)
 {
-    const int    b0 = ctl[self], b1 = ctl[self + 1];
-    const size_t first = (size_t)4 * b0 * W, last = (size_t)min(4 * b1, H) * W;
-    const size_t a0 = min((first + 15) & ~(size_t)15, last), a1 = max(last & ~(size_t)15, a0); // 16-byte aligned body [a0, a1)
-    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
-    const uint8_t* src = counts.p[self];
+    const size_t a0 = min((first + 15) & ~(size_t)15, last), a1 = max(last & ~(size_t)15, a0);
     for (size_t i = a0 / 16 + tid; i < a1 / 16; i += nthr)
     {
         const uint4 v = reinterpret_cast<const uint4*>(src)[i];
         for (int r = 0; r < world; r++)
-            if (r != self) reinterpret_cast<uint4*>(counts.p[r])[i] = v;
+            if (r != self && dst.p[r]) reinterpret_cast<uint4*>(dst.p[r])[i] = v;
     }
     if (tid < 32)
     {
-        const size_t i = tid < 16 ? first + tid : a1 + (tid - 16); // head: [first, a0), tail: [a1, last), 15 bytes at most each
+        const size_t i = tid < 16 ? first + tid : a1 + (tid - 16);
         if (i < (tid < 16 ? a0 : last))
         {
             const uint8_t v = src[i];
             for (int r = 0; r < world; r++)
-                if (r != self) counts.p[r][i] = v;
+                if (r != self && dst.p[r]) dst.p[r][i] = v;
         }
     }
+}
+
+__global__ void __launch_bounds__(256) k_rt_push_count(CountPtrs counts, CostPtrs costs, int* __restrict__ ctl, uint32_t* __restrict__ acc, TickPtrs ticks, int world,
+                                                       int self, int parity, int MH, int W, int H, int tick)
+{
+    const int    b0 = ctl[self], b1 = ctl[self + 1];
+    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
+    push_bytes(counts.p[self], counts, world, self, (size_t)4 * b0 * W, (size_t)min(4 * b1, H) * W, tid, nthr);
     // the cost drain and the tick: as in k_rt_push
     if (blockIdx.x == 0)
         for (int row = b0 + threadIdx.x; row < b1; row += blockDim.x)
@@ -451,21 +442,15 @@ void hr_peer_register(hr_pass* p, void* const* imgs, int n)
     for (int k = 0; k < n; k++) p->hist_local[k] = imgs[k];
 }
 
-// Collective over the NCCL communicator: all-gather the CUDA IPC handles of this pass's history images and tick array,
-// map every peer's.  Called from the first sharded render of the pass (all ranks render their passes in the same order).
-int hr_peer_link_ipc(hr_pass* p, cudaStream_t st)
+// Collective over the NCCL communicator: all-gather the CUDA IPC handles of the `n` allocations local[] of every rank and map the
+// peers': out[r * n + k] = rank r's allocation k in this process (local[k] for r == self).
+static int ipc_exchange(hr_ctx* ctx, void* const* local, int n, void** out, cudaStream_t st)
 {
-    hr_ctx* ctx = p->ctx;
-    if (p->peers_linked || ctx->world <= 1 || !ctx->nccl_comm || p->n_hist == 0) return HR_OK;
-    NcclApi& N = nccl();
-    int      rc = peer_alloc_ticks(p);
-    if (rc == HR_OK) rc = rt_alloc_counts(p);
-    if (rc != HR_OK) return rc;
-    const int    nh = p->n_hist + 1, world = ctx->world;
-    const size_t hb = sizeof(cudaIpcMemHandle_t), mine = hb * nh;
-    std::vector<cudaIpcMemHandle_t> h(nh), all((size_t)nh * world);
-    for (int k = 0; k < p->n_hist; k++) HR_CUDA(ctx, cudaIpcGetMemHandle(&h[k], p->hist_local[k]));
-    HR_CUDA(ctx, cudaIpcGetMemHandle(&h[p->n_hist], p->sync_ticks));
+    NcclApi&     N = nccl();
+    const int    world = ctx->world;
+    const size_t mine  = sizeof(cudaIpcMemHandle_t) * n;
+    std::vector<cudaIpcMemHandle_t> h(n), all((size_t)n * world);
+    for (int k = 0; k < n; k++) HR_CUDA(ctx, cudaIpcGetMemHandle(&h[k], local[k]));
     char *d_send = nullptr, *d_recv = nullptr;
     HR_CUDA(ctx, cudaMalloc((void**)&d_send, mine));
     HR_CUDA(ctx, cudaMalloc((void**)&d_recv, mine * world));
@@ -476,20 +461,34 @@ int hr_peer_link_ipc(hr_pass* p, cudaStream_t st)
     cudaFree(d_send);
     cudaFree(d_recv);
     for (int r = 0; r < world; r++)
+        for (int k = 0; k < n; k++)
+        {
+            void*& m = out[(size_t)r * n + k];
+            if (r == ctx->rank) m = local[k];
+            else HR_CUDA(ctx, cudaIpcOpenMemHandle(&m, all[(size_t)r * n + k], cudaIpcMemLazyEnablePeerAccess));
+        }
+    return HR_OK;
+}
+
+// Collective: map every peer's shared images and tick array.  Called from the first sharded render of the pass (all ranks render their
+// passes in the same order).
+int hr_peer_link_ipc(hr_pass* p, cudaStream_t st)
+{
+    hr_ctx* ctx = p->ctx;
+    if (p->peers_linked || ctx->world <= 1 || !ctx->nccl_comm || p->n_hist == 0) return HR_OK;
+    int rc = peer_alloc_ticks(p);
+    if (rc == HR_OK) rc = rt_alloc_counts(p);
+    if (rc != HR_OK) return rc;
+    const int nh = p->n_hist + 1;
+    void*     local[HR_MAX_SHARED + 1];
+    void*     all[HR_MAX_RANKS * (HR_MAX_SHARED + 1)];
+    for (int k = 0; k < p->n_hist; k++) local[k] = p->hist_local[k];
+    local[p->n_hist] = p->sync_ticks;
+    if ((rc = ipc_exchange(ctx, local, nh, all, st)) != HR_OK) return rc;
+    for (int r = 0; r < ctx->world; r++)
     {
-        if (r == ctx->rank)
-        {
-            for (int k = 0; k < p->n_hist; k++) p->hist_peer[r][k] = p->hist_local[k];
-            p->peer_ticks[r] = p->sync_ticks;
-            continue;
-        }
-        for (int k = 0; k < nh; k++)
-        {
-            void* m = nullptr;
-            HR_CUDA(ctx, cudaIpcOpenMemHandle(&m, all[(size_t)r * nh + k], cudaIpcMemLazyEnablePeerAccess));
-            if (k < p->n_hist) p->hist_peer[r][k] = m;
-            else p->peer_ticks[r] = (int*)m;
-        }
+        for (int k = 0; k < p->n_hist; k++) p->hist_peer[r][k] = all[r * nh + k];
+        p->peer_ticks[r] = static_cast<int*>(all[r * nh + p->n_hist]);
     }
     if (p->rt_bounds) { rc = rt_init_bounds(p); if (rc != HR_OK) return rc; }
     p->peers_linked = true;
@@ -499,6 +498,7 @@ int hr_peer_link_ipc(hr_pass* p, cudaStream_t st)
 
 void hr_peer_unlink(hr_pass* p)
 {
+    hr_ddgi_unmap(p);
     if (p->peers_ipc)
         for (int r = 0; r < HR_MAX_RANKS; r++)
         {
@@ -585,6 +585,130 @@ int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* n
     }
     const int n_chunks = (p->H + 7) / 8, mine = (n_chunks - ctx->rank + ctx->world - 1) / ctx->world;
     k_rt_push_chunks<<<(mine > 0 ? mine : 1) * PUSH_SPLIT, 256, 0, st>>>(im, nd, t, p->rt_bounds, ctx->world, ctx->rank, p->W, p->H, tick);
+    ctx->launches++;
+    return HR_OK;
+}
+
+// ---- DDGI atlases -----------------------------------------------------------------------------------------------------
+// Linked DDGI passes split the probe stages by z-slices (hr_api_gi.inc).  The slices of a rank are one contiguous row range of each
+// atlas, which the rank stores into every peer's atlas of this frame's ping-pong after its K19/K20 (k_ddgi_push), so every rank
+// holds the complete atlases without a collective on the render stream.  The atlases are allocated when the grid is (re)initialised,
+// after the passes were linked, so the push reads the peers' addresses at run time from this rank's table (shared image 0,
+// [rank][irradiance 0, irradiance 1, depth 0, depth 1]):
+//   * same-process ranks render one after another from one thread, so rank 0 enqueues the push of a re-initialisation frame before
+//     rank 1 has allocated its new atlases.  After a (re)initialisation every rank writes its addresses into its peers' tables on
+//     its stream and then publishes its ready tick (slot 1) = that render's frame tick (k_ddgi_publish); in that render the push
+//     is preceded by a one-warp wait until every peer's ready tick reached it (hr_api_gi.inc).
+//   * IPC ranks re-initialise in the same render (they render the same scene with the same parameters): they exchange the new
+//     atlases' IPC handles in a collective and write the mapped addresses into their own table; the push waits for nothing.
+// One frame tick (slot 0) orders the stores: a rank publishes tick N after its frame-N stores (last block of k_ddgi_push) and waits,
+// before its K21, until every peer's tick reached N.
+//   * Write before read: K21 and the reflections of frame N read atlas[mp] after that wait, so it is complete.
+//   * Read before write: the frame-N stores go into atlas[mp], which a peer last read in frame N-1 (K18's infinite bounce, every
+//     probe; K19's hysteresis, its slices) and, before that, in frame N-2 (its K21 and reflections).  This rank's frame-N push runs
+//     after its frame N-1 wait saw that peer's tick N-1, which the peer published after its frame N-1 K18 and K19 and, in stream
+//     order, after its frame N-2 consumers — as long as every consumer of the atlas runs on the render stream.
+namespace {
+
+struct AtlasSet { void* a[4]; };
+struct TabPtrs { void** p[HR_MAX_RANKS]; };
+struct BytePtrs { uint8_t* const* p; };
+
+__global__ void k_ddgi_publish(TabPtrs tabs, TickPtrs ticks, AtlasSet mine, int world, int self, int tick)
+{
+    const int r = threadIdx.x;
+    if (r >= world || r == self || !tabs.p[r] || !ticks.p[r]) return;
+    for (int k = 0; k < 4; k++) tabs.p[r][self * 4 + k] = mine.a[k];
+    __threadfence_system();
+    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
+}
+
+// Bytes [i0, i1) of the irradiance atlas and [d0, d1) of the depth atlas (ping-pong mp) into every peer's atlas, at the addresses in
+// this rank's table; the last block publishes the atlas tick.
+__global__ void __launch_bounds__(256) k_ddgi_push(void* const* tab, const uint8_t* __restrict__ irr, const uint8_t* __restrict__ dep, size_t i0, size_t i1, size_t d0,
+                                                   size_t d1, int mp, TickPtrs peers, int* __restrict__ ctl, int world, int self, int tick)
+{
+    __shared__ uint8_t* s_dst[2][HR_MAX_RANKS];
+    const int r = threadIdx.x;
+    if (r < HR_MAX_RANKS)
+    { // written by the peer before its ready tick (same process), or by this rank's host at the grid's initialisation (IPC)
+        const bool peer = r < world && r != self;
+        s_dst[0][r] = peer ? static_cast<uint8_t*>(*reinterpret_cast<void* const volatile*>(tab + r * 4 + mp)) : nullptr;
+        s_dst[1][r] = peer ? static_cast<uint8_t*>(*reinterpret_cast<void* const volatile*>(tab + r * 4 + 2 + mp)) : nullptr;
+    }
+    __syncthreads();
+    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
+    push_bytes(irr, BytePtrs { s_dst[0] }, world, self, i0, i1, tid, nthr);
+    push_bytes(dep, BytePtrs { s_dst[1] }, world, self, d0, d1, tid, nthr);
+    __threadfence_system();
+    __syncthreads();
+    __shared__ int s_last;
+    if (threadIdx.x == 0) s_last = atomicAdd(ctl + HR_MAX_RANKS + 2, 1) == (int)gridDim.x - 1;
+    __syncthreads();
+    if (!s_last) return;
+    if (threadIdx.x == 0) ctl[HR_MAX_RANKS + 2] = 0; // blocks-done counter
+    if (r < world && r != self && peers.p[r])
+    {
+        __threadfence_system(); // all blocks' stores (ordered before their atomicAdd) are visible before the tick
+        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(peers.p[r] + self), "r"(tick) : "memory");
+    }
+}
+
+} // namespace
+
+void hr_ddgi_unmap(hr_pass* p)
+{
+    for (int r = 0; r < HR_MAX_RANKS; r++)
+        for (int k = 0; k < 4; k++)
+            if (p->ddgi_mapped[r][k])
+            {
+                cudaIpcCloseMemHandle(p->ddgi_mapped[r][k]);
+                p->ddgi_mapped[r][k] = nullptr;
+            }
+}
+
+int hr_ddgi_publish(hr_pass* p, int tick, cudaStream_t st)
+{
+    hr_ctx* ctx  = p->ctx;
+    AtlasSet mine { { p->ddgi_irr[0], p->ddgi_irr[1], p->ddgi_depth[0], p->ddgi_depth[1] } };
+    if (p->peers_ipc)
+    {
+        void* all[HR_MAX_RANKS * 4];
+        int   rc = ipc_exchange(ctx, mine.a, 4, all, st);
+        if (rc != HR_OK) return rc;
+        for (int r = 0; r < ctx->world; r++)
+            for (int k = 0; k < 4 && r != ctx->rank; k++) p->ddgi_mapped[r][k] = all[r * 4 + k];
+        HR_CUDA(ctx, cudaMemcpyAsync(p->ddgi_tab, all, sizeof(void*) * 4 * ctx->world, cudaMemcpyHostToDevice, st));
+        HR_CUDA(ctx, cudaStreamSynchronize(st));
+        // The replaced atlases: every peer's stores into them completed before this render (this rank's stream passed its last atlas
+        // wait, which saw every peer's tick published after its stores, and was synchronised at the re-initialisation), and every peer
+        // closed its mappings of them before it entered the exchange above (hr_ddgi_unmap at its re-initialisation).
+        for (void* a : p->ddgi_retired) cudaFree(a);
+        p->ddgi_retired.clear();
+    }
+    else
+    {
+        TabPtrs  t {};
+        TickPtrs k {};
+        for (int r = 0; r < ctx->world; r++)
+        {
+            t.p[r] = static_cast<void**>(p->hist_peer[r][0]);
+            k.p[r] = p->peer_ticks[r];
+        }
+        k_ddgi_publish<<<1, 32, 0, st>>>(t, k, mine, ctx->world, ctx->rank, tick);
+        ctx->launches++;
+    }
+    p->ddgi_ready = tick;
+    return HR_OK;
+}
+
+int hr_ddgi_push(hr_pass* p, int mp, size_t i0, size_t i1, size_t d0, size_t d1, int tick, cudaStream_t st)
+{
+    hr_ctx* ctx = p->ctx;
+    TickPtrs t {};
+    for (int r = 0; r < ctx->world; r++) t.p[r] = p->peer_ticks[r];
+    k_ddgi_push<<<ctx->sm_count, 256, 0, st>>>(p->ddgi_tab, (const uint8_t*)p->ddgi_irr[mp], (const uint8_t*)p->ddgi_depth[mp], i0, i1, d0, d1, mp, t, p->rt_bounds,
+                                               ctx->world, ctx->rank, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -685,6 +809,32 @@ int hr_shard_init(hr_ctx* ctx, int rank, int world, const void* unique_id_128_by
     return HR_OK;
 }
 
+// Same-process DDGI ranks allocate their grids from a pool of their own, in stream order (hr_api_gi.inc).  `pass`'s rank stores into `peer`'s
+// atlases, so a peer on another device grants this rank's device access to its pool (pool memory is not covered by peer access).
+static int ddgi_pool_create(hr_pass* p)
+{
+    if (p->ddgi_pool) return HR_OK;
+    cudaMemPoolProps props {};
+    props.allocType     = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id   = p->ctx->device;
+    HR_CUDA(p->ctx, cudaMemPoolCreate(&p->ddgi_pool, &props));
+    return HR_OK;
+}
+
+static int ddgi_pool_link(hr_pass* pass, hr_pass* peer)
+{
+    int rc = ddgi_pool_create(pass);
+    if (rc == HR_OK) rc = ddgi_pool_create(peer);
+    if (rc != HR_OK || pass->ctx->device == peer->ctx->device) return rc;
+    cudaMemAccessDesc a {};
+    a.location.type = cudaMemLocationTypeDevice;
+    a.location.id   = pass->ctx->device;
+    a.flags         = cudaMemAccessFlagsProtReadWrite;
+    HR_CUDA(pass->ctx, cudaMemPoolSetAccess(peer->ddgi_pool, &a, 1));
+    return HR_OK;
+}
+
 // Same-process peers (N ranks emulated on one GPU, or a multi-GPU single-process host): rank `rank`'s history lives in
 // `peer`'s images.  Every pass of the group must be linked with every other before the first sharded render.
 int hr_shard_link_local(hr_pass* pass, int rank, hr_pass* peer)
@@ -698,6 +848,7 @@ int hr_shard_link_local(hr_pass* pass, int rank, hr_pass* peer)
     if (rc == HR_OK) rc = peer_alloc_ticks(peer);
     if (rc == HR_OK) rc = rt_alloc_counts(pass);
     if (rc == HR_OK) rc = rt_alloc_counts(peer);
+    if (rc == HR_OK && pass->kind == PASS_DDGI) rc = ddgi_pool_link(pass, peer);
     if (rc != HR_OK) return rc;
     for (int k = 0; k < pass->n_hist; k++) pass->hist_peer[rank][k] = peer->hist_local[k];
     pass->peer_ticks[rank] = peer->sync_ticks;

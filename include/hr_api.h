@@ -379,7 +379,14 @@ HR_API int  hr_ddgi_create(hr_ctx* ctx, int width, int height, int scale, hr_pas
  * when probe_distance / irradiance_oct_size / depth_oct_size / rays_per_probe change, and after a failed initialisation
  * (ddgi.cpp:150-169).  A re-initialised grid starts like the first frame: zero atlases, no hysteresis, no infinite bounce.  The
  * other parameters are applied every frame.  Out-of-range parameters return HR_ERR_INVALID_ARG and change nothing; a grid of
- * more than 2^20 probes returns HR_ERR_UNSUPPORTED and leaves the pass without a grid (the next render initialises one). */
+ * more than 2^20 probes returns HR_ERR_UNSUPPORTED and leaves the pass without a grid (the next render initialises one).
+ * Sharded (world > 1): linked to its peers (hr_shard_init, or hr_shard_link_local for ranks of one process) rank r traces and updates
+ * the probes of the z-slices [cz * r / world, cz * (r + 1) / world) and stores their atlas rows into every peer's atlases, so outputs 2
+ * and 3 are complete on every rank once the stream passes the render; the per-pixel sample (output 4 / 100) covers the rank's band.
+ * Consumers of the atlases (hr_reflections_render, downloads) must run on the render stream, and all ranks must re-initialise their
+ * grids in the same render; the replaced grid is freed in that render (same-process ranks: in stream order on the render stream), so
+ * re-initialisations do not accumulate memory.  Not linked (hr_shard_config only): every probe on every rank.  Outputs 0 and 1 hold the
+ * rank's probes. */
 HR_API int hr_ddgi_render(hr_pass* pass, const hr_frame* frame, const hr_ddgi_params* params, const float* random_orientation16, void* stream);
 /* The uniforms of the current grid; HR_ERR_NOT_READY before the first render and after a failed grid initialisation. */
 HR_API int hr_ddgi_get_uniforms(hr_pass* pass, hr_ddgi_uniforms* out);
@@ -603,7 +610,8 @@ HR_API int hr_shard_set_gather(hr_ctx* ctx, int gather_final_output);
 #define HR_PASS_KIND_REFLECTIONS 3
 HR_API int hr_shard_halo_rows(int pass_kind, int radius, int filter_iterations, int blur_radius, int* denoise_halo, int* ray_trace_halo);
 /* Same-process peers (N ranks emulated on one GPU with hr_shard_config, or several GPUs driven by one process): declare
- * that rank `rank`'s band of this pass's history lives in `peer`.  Link every pass with every other rank's pass before
+ * that rank `rank`'s band of this pass's history lives in `peer` (DDGI: that `peer` receives this rank's probe slices).  Passes of
+ * another kind or size are refused.  Link every pass with every other rank's pass before
  * the first render, give every rank its own stream (the ranks wait for each other's ray masks inside a frame, so their
  * kernels must be able to run concurrently) and run the process with CUDA_MODULE_LOADING=EAGER (a lazily loaded kernel's
  * first launch synchronises the context, which stalls until the peer time-out while another rank's wait kernel spins). */
