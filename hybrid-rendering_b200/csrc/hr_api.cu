@@ -721,7 +721,7 @@ static void pass_alloc_rt_share(PassAllocs& A)
     A(p->mask_pp[1], mw * mh);
     A(p->rt_cost_all, 2 * mh);
     A(p->rt_cost_acc, mh);
-    A(p->rt_bounds, (size_t)HR_MAX_RANKS + 4); // + job counter, push-blocks-done counter
+    A(p->rt_bounds, (size_t)HR_CTL_WORDS);
 }
 
 static void set_view(hr_pass* p, int which, void* ptr, int w, int h, int fmt) { p->out_view[which] = { ptr, w, h, fmt }; }
@@ -833,7 +833,7 @@ static int frame_begin(hr_pass* p, const hr_frame* f, bool denoise, const HaloPl
 static int frame_signal(hr_pass* p, PassFrame& fr)
 {
     fr.signalled = true;
-    return hr_peer_signal(p, 0, fr.epoch, fr.st);
+    return hr_peer_signal(p, TICK_HIST, fr.epoch, fr.st);
 }
 
 static int frame_end(hr_pass* p, PassFrame& fr)
@@ -893,7 +893,7 @@ static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const 
         timer_mark(p, "Ray Trace", fr.st);
         // the history = last frame's images of whichever rank owns the reprojected row (peer history, shard.cu): wait until every
         // peer has finished writing them (tick epoch - 1), overlapped with the ray trace above
-        if (denoise && !fr.no_history && (rc = hr_peer_wait(p, 0, fr.epoch - 1, fr.st)) != HR_OK) return rc;
+        if (denoise && !fr.no_history && (rc = hr_peer_wait(p, TICK_HIST, fr.epoch - 1, fr.st)) != HR_OK) return rc;
     }
     if (spp > 1) fr.final = { count, p->W, p->H, HR_FMT_R8_UINT };
     else fr.final = { mask, (p->W + 7) / 8, (p->H + 3) / 4, HR_FMT_R32_UINT };
@@ -953,8 +953,9 @@ int hr_shadows_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** o
         A(p->tile_flags, tw * th);
         if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
         pass_alloc_rt_share(A);
-        void* hist[9] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all, p->count_pp[0], p->count_pp[1] };
-        hr_peer_register(p, hist, 9);
+        void* hist[SHARED_N_SHADOWS_AO] = { p->prev_image[0], p->prev_image[1], p->moments[0], p->moments[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all,
+                                            p->count_pp[0], p->count_pp[1] };
+        hr_peer_register(p, hist, SHARED_N_SHADOWS_AO);
         for (int i = 0; i < 2; i++)
         {
             p->hist_view[HR_SHADOWS_OUT_PREV_IMAGE][i] = { p->prev_image[i], p->W, p->H, HR_FMT_RG16F };
@@ -999,7 +1000,7 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
         // temporal_accumulation (:1041-1090); reset_args (:1015-1037) is subsumed by the per-tile flag image.
         // History = prev_image[!pp] / moments[!pp] of whichever rank owns the reprojected row (peer history, shard.cu).
         HistPeers hist;
-        hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
+        hr_peer_hist(p, SHARED_HIST + !pp, SHARED_HIST_AUX + !pp, p->H, fr.no_history, &hist);
         if (spp > 1)
             launch_shadows_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
         else
@@ -1089,8 +1090,9 @@ int hr_ao_create(hr_ctx* ctx, int width, int height, int scale, hr_pass** out)
         A(p->tile_flags, tw * th);
         if (p->scale != HR_SCALE_FULL) A(p->upsample_out, (size_t)p->W0 * p->H0);
         pass_alloc_rt_share(A);
-        void* hist[9] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all, p->count_pp[0], p->count_pp[1] };
-        hr_peer_register(p, hist, 9);
+        void* hist[SHARED_N_SHADOWS_AO] = { p->ao_color[0], p->ao_color[1], p->ao_len[0], p->ao_len[1], p->mask_pp[0], p->mask_pp[1], p->rt_cost_all,
+                                            p->count_pp[0], p->count_pp[1] };
+        hr_peer_register(p, hist, SHARED_N_SHADOWS_AO);
         for (int i = 0; i < 2; i++)
         {
             p->hist_view[HR_AO_OUT_TEMPORAL_ACCUMULATION][i] = { p->ao_color[i], p->W, p->H, HR_FMT_R16F };
@@ -1130,7 +1132,7 @@ int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* s
     {
         // history = ao_color[!pp] / ao_len[!pp] of the rank that owns the reprojected row (peer history, shard.cu)
         HistPeers hist;
-        hr_peer_hist(p, !pp, 2 + !pp, p->H, fr.no_history, &hist);
+        hr_peer_hist(p, SHARED_HIST + !pp, SHARED_HIST_AUX + !pp, p->H, fr.no_history, &hist);
         if (spp > 1) launch_ao_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         else launch_ao_temporal(cur, prev, mask, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;

@@ -58,6 +58,34 @@ struct FrameConsts {           // what kernels need from hr_frame (passed by val
 #define HR_MAX_RANKS 8
 #define HR_MAX_SHARED 9
 
+// Shared images of a pass (hr_peer_register order, the index of hist_local / hist_peer), by pass kind.  History images come in pairs by
+// G-buffer parity; the ray-trace images of the cooperative trace in pairs by frame parity.
+enum SharedImage {
+    SHARED_HIST = 0,     // shadows, AO, reflections: temporal history (shadows prev_image, AO colour, reflections current output) [2]
+    SHARED_HIST_AUX = 2, //   and its companion (shadows and reflections moments, AO history length) [2]
+    SHARED_MASK = 4,     // shadows, AO: ray mask [2]
+    SHARED_COST = 6,     //   ray-trace cost table [2][mask rows]
+    SHARED_COUNT = 7,    //   spp > 1 count image [2] (null until the pass is linked)
+    SHARED_N_SHADOWS_AO = 9,
+    SHARED_RT = 4,       // reflections: ray-trace output [2]
+    SHARED_N_REFLECTIONS = 6,
+    SHARED_PT_IMG = 0,   // path tracer: the two accumulation images
+    SHARED_N_PATH_TRACER = 2,
+    SHARED_DDGI_TAB = 0, // DDGI: the peers' atlas addresses [rank][irradiance 0, 1, depth 0, 1]
+    SHARED_N_DDGI = 1,
+};
+
+// The two frame-tick slots of a linked pass: sync_ticks[slot][rank] is written by rank `rank` into this rank's memory.
+//   shadows, AO, reflections: TICK_HIST = the history images of that frame are complete; TICK_RT = the frame's ray-trace share is pushed.
+//   path tracer: TICK_RT = the render's chunks are pushed.
+//   DDGI: TICK_ATLAS (slot 0) = the frame's atlas slices are pushed; TICK_DDGI_READY (slot 1) = the current atlases' addresses are published.
+enum TickSlot { TICK_HIST = 0, TICK_RT = 1, TICK_ATLAS = 0, TICK_DDGI_READY = 1 };
+
+// Control block of a linked pass (hr_pass::rt_bounds): [0, world] the mask-row partition of the next frame's ray trace (shadows, AO),
+// then the count of blocks of the running push kernel that are done.
+#define HR_CTL_BLOCKS_DONE (HR_MAX_RANKS + 1)
+#define HR_CTL_WORDS (HR_MAX_RANKS + 2)
+
 // Temporal history as the reprojection kernels see it (shard.cu, "peer history").  Row y of the previous frame's history
 // images lives on the rank that owns y (band_end[r] = first row NOT owned by ranks 0..r); img[r] / aux[r] are that rank's
 // full-size images — this GPU's own for r == self, NVLink peer mappings (CUDA IPC) otherwise.  Single GPU: world = 1.
@@ -240,16 +268,15 @@ struct hr_pass {
     // peer history (shard.cu): the history images of every rank mapped into this process, and the frame ticks that order
     // "rank q finished writing frame N's history" before "rank r's frame N+1 reprojection reads it"
     bool        peers_linked = false, peers_ipc = false;
-    int         n_hist = 0;                          // shared images: 0-3 history (shadows: prev_image[2], moments[2]; AO: colour[2], length[2]),
-                                                     // 4-5 ray mask [frame parity], 6 ray-trace cost table [2][mask rows], 7-8 count image [frame parity] (null until linked)
+    int         n_hist = 0;                          // shared images (SharedImage)
     void*       hist_local[HR_MAX_SHARED] = {};
     void*       hist_peer[HR_MAX_RANKS][HR_MAX_SHARED] = {}; // [rank][image]; own rank = hist_local
-    int*        sync_ticks = nullptr;                // [2][HR_MAX_RANKS] ticks written by the peers into THIS rank's memory: [0] history, [1] ray trace
+    int*        sync_ticks = nullptr;                // [2][HR_MAX_RANKS] ticks written by the peers into THIS rank's memory (TickSlot)
     uint32_t*   mask_pp[2] = { nullptr, nullptr };   // ray mask by frame parity (mask_pp[0] == mask); peers push their rows into both copies' owner
     uint8_t*    count_pp[2] = { nullptr, nullptr };  // spp > 1 on linked ranks: the count image by frame parity, pushed like mask_pp (allocated at link time)
     uint32_t*   rt_cost_all = nullptr;               // [2][MH] per-mask-row trace cost of the frame (all ranks' rows, pushed by their owners)
     uint32_t*   rt_cost_acc = nullptr;               // [MH] this rank's accumulation scratch (atomicAdd per warp), drained by the push kernel
-    int*        rt_bounds = nullptr;                 // [world+1] mask-row partition of the NEXT frame's ray trace (device side, cost balanced); [HR_MAX_RANKS+1] = job counter, [+2] = push blocks done
+    int*        rt_bounds = nullptr;                 // control block [HR_CTL_WORDS]: [world+1] mask-row partition of the NEXT frame's ray trace (device side, cost balanced), push blocks done
     int*        peer_ticks[HR_MAX_RANKS] = {};       // the peers' tick arrays (we write slot [self])
     int*        sync_error = nullptr;                // set by the wait kernel on time-out
     int         epoch = 0;                           // renders of this pass so far
@@ -286,10 +313,12 @@ struct ExchangeItem { void* base; size_t row_bytes; int H; int shift; int div; i
 // peer history (shard.cu)
 void hr_peer_register(hr_pass* p, void* const* imgs, int n);
 int  hr_peer_link_ipc(hr_pass* p, cudaStream_t st);
+// The pass renders as one of `world` linked ranks (hr_shard_init + hr_peer_link_ipc, or hr_shard_link_local).
+inline bool hr_peer_linked(const hr_pass* p) { return p->ctx->world > 1 && p->peers_linked; }
 void hr_peer_unlink(hr_pass* p);
 void hr_peer_hist(const hr_pass* p, int img_k, int aux_k, int H, bool no_history, HistPeers* out);
-int  hr_peer_wait(hr_pass* p, int which, int tick, cudaStream_t st);   // which: 0 history ticks, 1 ray-trace ticks
-int  hr_peer_signal(hr_pass* p, int which, int tick, cudaStream_t st);
+int  hr_peer_wait(hr_pass* p, int slot, int tick, cudaStream_t st); // slot: TickSlot
+int  hr_peer_signal(hr_pass* p, int slot, int tick, cudaStream_t st);
 // Cost-balanced ray trace over the whole image with the masks pushed to every peer (trace.cu / shard.cu).
 struct RtShare {
     uint32_t*     mask_local; // this rank's mask image of this frame's parity (k_rt_push copies the share to the peers)
@@ -308,7 +337,7 @@ int  hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cu
 int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* need1, cudaStream_t st); // img: the shared image (hr_peer_register index)
 // DDGI atlases of linked ranks (shard.cu): after a grid (re)initialisation, make this rank's atlas addresses known to its peers (IPC ranks:
 // a collective that maps the peers' new atlases, then frees the replaced atlases); after K19/K20, store bytes [i0, i1) of the irradiance and
-// [d0, d1) of the depth atlas of ping-pong mp into every peer's atlas and publish the atlas tick `tick` (hr_peer_wait slot 0).
+// [d0, d1) of the depth atlas of ping-pong mp into every peer's atlas and publish the atlas tick `tick` (slot TICK_ATLAS).
 int  hr_ddgi_publish(hr_pass* p, int tick, cudaStream_t st);
 int  hr_ddgi_push(hr_pass* p, int mp, size_t i0, size_t i1, size_t d0, size_t d1, int tick, cudaStream_t st);
 void hr_ddgi_unmap(hr_pass* p); // close the IPC mappings of the peers' atlases

@@ -139,91 +139,81 @@ static int rt_init_bounds(hr_pass* p);
 
 namespace {
 
-struct TickPtrs { int* p[HR_MAX_RANKS]; };
+// One pointer per rank: a shared image or tick array of every rank as this process sees it.
+template <class T> struct PeerPtrs { T* p[HR_MAX_RANKS]; };
 
-__global__ void k_peer_signal(TickPtrs peers, int world, int self, int slot, int tick)
+// The peers' tick arrays (a pass's tick publications write slot [self] of each).
+PeerPtrs<int> peer_tick_ptrs(const hr_pass* p)
 {
-    const int r = threadIdx.x;
-    if (r >= world || r == self || !peers.p[r]) return;
-    __threadfence_system(); // the writes of the kernels before us in stream order become visible system-wide first
-    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(peers.p[r] + slot * HR_MAX_RANKS + self), "r"(tick) : "memory");
+    PeerPtrs<int> t {};
+    for (int r = 0; r < p->ctx->world; r++) t.p[r] = p->peer_ticks[r];
+    return t;
 }
 
-// ---- cooperative ray trace: push of the traced share + cost-balanced partition ----
-struct CostPtrs { uint32_t* p[HR_MAX_RANKS]; };
-struct MaskPtrs { uint32_t* p[HR_MAX_RANKS]; };
-
-// After the ray-trace kernel: copy this rank's share of the mask image (rows [bounds[self], bounds[self+1])) into every
-// peer's mask image with wide stores, drain the cost accumulation into every rank's cost table, reset the job counter,
-// and — from the last block to finish — publish the ray-trace tick to the peers.
-__global__ void __launch_bounds__(256) k_rt_push(MaskPtrs masks, CostPtrs costs, int* __restrict__ ctl, uint32_t* __restrict__ acc, TickPtrs ticks, int world, int self,
-                                                 int parity, int MH, int MW, int tick)
+// Shared image k (SharedImage) of every rank.
+template <class T> PeerPtrs<T> peer_image_ptrs(const hr_pass* p, int k)
 {
-    const int    b0 = ctl[self], b1 = ctl[self + 1];
-    const size_t first = (size_t)b0 * MW, n = (size_t)(b1 - b0) * MW;
-    const uint32_t* src = masks.p[self] + first;
-    const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
-    if ((MW & 3) == 0)
-    { // rows are 16-byte multiples and the images 256-byte aligned
-        const uint4* s4 = reinterpret_cast<const uint4*>(src);
-        for (size_t i = tid; i < n / 4; i += nthr)
-        {
-            const uint4 v = s4[i];
-            for (int r = 0; r < world; r++)
-                if (r != self) reinterpret_cast<uint4*>(masks.p[r] + first)[i] = v;
-        }
+    PeerPtrs<T> m {};
+    for (int r = 0; r < p->ctx->world; r++) m.p[r] = static_cast<T*>(p->hist_peer[r][k]);
+    return m;
+}
+
+__device__ __forceinline__ void st_release_sys(int* a, int v) { asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(a), "r"(v) : "memory"); }
+
+// Lane r (a peer) spins until its tick `*t` reached `tick`.  After 10 s it gives up and sets *err = 1 + r: a peer died or the ranks
+// render different frame counts, and the GPU must not hang.  Returns false on a time-out.
+__device__ __forceinline__ bool wait_tick(const int* t, int r, int tick, int* err, unsigned sleep_ns)
+{
+    unsigned long long t0, t1;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    for (;;)
+    {
+        int v;
+        asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(t) : "memory");
+        if (v >= tick) return true;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+        if (t1 - t0 > 10000000000ull) { *err = 1 + r; return false; }
+        __nanosleep(sleep_ns);
     }
-    else
-        for (size_t i = tid; i < n; i += nthr)
-        {
-            const uint32_t v = src[i];
-            for (int r = 0; r < world; r++)
-                if (r != self) masks.p[r][first + i] = v;
-        }
-    if (blockIdx.x == 0)
-        for (int row = b0 + threadIdx.x; row < b1; row += blockDim.x)
-        {
-            const uint32_t v = acc[row];
-            acc[row]         = 0u;
-            for (int r = 0; r < world; r++) costs.p[r][(size_t)parity * MH + row] = v;
-        }
+}
+
+// The end of a push kernel: every block makes its stores visible system-wide and counts itself done; the last block resets the
+// counter and publishes `tick` in slot `slot` of every peer's tick array.
+__device__ __forceinline__ void publish_when_grid_done(int* __restrict__ ctl, const PeerPtrs<int>& ticks, int world, int self, int slot, int tick)
+{
     __threadfence_system();
     __syncthreads();
     __shared__ int s_last;
-    if (threadIdx.x == 0)
-    {
-        const int done = atomicAdd(ctl + HR_MAX_RANKS + 2, 1);
-        s_last         = done == (int)gridDim.x - 1;
-    }
+    if (threadIdx.x == 0) s_last = atomicAdd(ctl + HR_CTL_BLOCKS_DONE, 1) == (int)gridDim.x - 1;
     __syncthreads();
     if (!s_last) return;
-    if (threadIdx.x == 0)
-    {
-        ctl[HR_MAX_RANKS + 2] = 0; // blocks-done counter
-    }
+    if (threadIdx.x == 0) ctl[HR_CTL_BLOCKS_DONE] = 0;
     const int r = threadIdx.x;
     if (r < world && r != self && ticks.p[r])
     {
         __threadfence_system(); // all blocks' stores (ordered before their atomicAdd) are visible before the tick
-        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
+        st_release_sys(ticks.p[r] + slot * HR_MAX_RANKS + self, tick);
     }
 }
 
-// spp > 1: k_rt_push for the count image (one byte per pixel): mask rows [b0, b1) are the image rows [4 * b0, min(4 * b1, H)), whose
-// byte range need not start or end on a 16-byte boundary (W is arbitrary), so the 16-byte body is framed by a byte-wise head and tail.
-struct CountPtrs { uint8_t* p[HR_MAX_RANKS]; };
+__global__ void k_peer_signal(PeerPtrs<int> peers, int world, int self, int slot, int tick)
+{
+    const int r = threadIdx.x;
+    if (r >= world || r == self || !peers.p[r]) return;
+    __threadfence_system(); // the writes of the kernels before us in stream order become visible system-wide first
+    st_release_sys(peers.p[r] + slot * HR_MAX_RANKS + self, tick);
+}
 
-// Bytes [first, last) of `src` to the same offsets of every peer's image dst.p[r] (r != self; null: skipped).  The images are 256-byte
+// Bytes [first, last) of `src` to the same offsets of every peer's image dst[r] (r != self; null: skipped).  The images are 256-byte
 // aligned, so a 16-byte body [a0, a1) is framed by a byte-wise head and tail of at most 15 bytes each, copied by threads 0-31 of the grid.
-template <class Ptrs>
-__device__ __forceinline__ void push_bytes(const uint8_t* __restrict__ src, const Ptrs& dst, int world, int self, size_t first, size_t last, size_t tid, size_t nthr)
+__device__ __forceinline__ void push_bytes(const uint8_t* __restrict__ src, uint8_t* const (&dst)[HR_MAX_RANKS], int world, int self, size_t first, size_t last, size_t tid, size_t nthr)
 {
     const size_t a0 = min((first + 15) & ~(size_t)15, last), a1 = max(last & ~(size_t)15, a0);
     for (size_t i = a0 / 16 + tid; i < a1 / 16; i += nthr)
     {
         const uint4 v = reinterpret_cast<const uint4*>(src)[i];
         for (int r = 0; r < world; r++)
-            if (r != self && dst.p[r]) reinterpret_cast<uint4*>(dst.p[r])[i] = v;
+            if (r != self && dst[r]) reinterpret_cast<uint4*>(dst[r])[i] = v;
     }
     if (tid < 32)
     {
@@ -232,18 +222,21 @@ __device__ __forceinline__ void push_bytes(const uint8_t* __restrict__ src, cons
         {
             const uint8_t v = src[i];
             for (int r = 0; r < world; r++)
-                if (r != self && dst.p[r]) dst.p[r][i] = v;
+                if (r != self && dst[r]) dst[r][i] = v;
         }
     }
 }
 
-__global__ void __launch_bounds__(256) k_rt_push_count(CountPtrs counts, CostPtrs costs, int* __restrict__ ctl, uint32_t* __restrict__ acc, TickPtrs ticks, int world,
-                                                       int self, int parity, int MH, int W, int H, int tick)
+// ---- cooperative ray trace: push of the traced share + cost-balanced partition ----
+// After the shadows / AO ray trace: copy this rank's share, mask rows [ctl[self], ctl[self + 1]), of the mask or count image to every
+// peer, drain the cost accumulation into every rank's cost table, and publish the ray-trace tick.  A mask row is `rows` image rows of
+// `row_bytes` bytes (mask image: 1 row of 4 * MW bytes; count image: 4 rows of W bytes), clamped to the image height H.
+__global__ void __launch_bounds__(256) k_rt_push(PeerPtrs<uint8_t> imgs, PeerPtrs<uint32_t> costs, int* __restrict__ ctl, uint32_t* __restrict__ acc,
+                                                 PeerPtrs<int> ticks, int world, int self, int parity, int MH, size_t row_bytes, int rows, int H, int tick)
 {
     const int    b0 = ctl[self], b1 = ctl[self + 1];
     const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
-    push_bytes(counts.p[self], counts, world, self, (size_t)4 * b0 * W, (size_t)min(4 * b1, H) * W, tid, nthr);
-    // the cost drain and the tick: as in k_rt_push
+    push_bytes(imgs.p[self], imgs.p, world, self, (size_t)rows * b0 * row_bytes, (size_t)min(rows * b1, H) * row_bytes, tid, nthr);
     if (blockIdx.x == 0)
         for (int row = b0 + threadIdx.x; row < b1; row += blockDim.x)
         {
@@ -251,30 +244,11 @@ __global__ void __launch_bounds__(256) k_rt_push_count(CountPtrs counts, CostPtr
             acc[row]         = 0u;
             for (int r = 0; r < world; r++) costs.p[r][(size_t)parity * MH + row] = v;
         }
-    __threadfence_system();
-    __syncthreads();
-    __shared__ int s_last;
-    if (threadIdx.x == 0)
-    {
-        const int done = atomicAdd(ctl + HR_MAX_RANKS + 2, 1);
-        s_last         = done == (int)gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!s_last) return;
-    if (threadIdx.x == 0)
-    {
-        ctl[HR_MAX_RANKS + 2] = 0; // blocks-done counter
-    }
-    const int r = threadIdx.x;
-    if (r < world && r != self && ticks.p[r])
-    {
-        __threadfence_system(); // all blocks' stores (ordered before their atomicAdd) are visible before the tick
-        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
-    }
+    publish_when_grid_done(ctl, ticks, world, self, TICK_RT, tick);
 }
 
-// One warp.  Lanes spin until every peer's ray-trace tick reached `rt_tick` and its history tick `hist_tick` (10 s time-out),
-// then the warp computes next frame's partition: bounds[k] = first mask row whose cost prefix reaches k/world of the total.
+// One warp.  Lanes wait until every peer's ray-trace tick reached `rt_tick` and its history tick `hist_tick`, then the warp computes
+// next frame's partition: bounds[k] = first mask row whose cost prefix reaches k/world of the total.
 // Every rank computes the same table from the same (complete) cost table.  Any height: each lane sums one 1/32 chunk of the
 // rows; a bound lies in the chunk of the first lane whose inclusive chunk prefix reaches its target, which the warp then scans
 // 32 rows at a time.
@@ -282,21 +256,8 @@ __global__ void k_rt_wait_partition(const int* __restrict__ ticks, int rt_tick, 
                                     int cap, int* __restrict__ bounds)
 {
     const int lane = threadIdx.x;
-    if (lane < world && lane != self)
-    {
-        unsigned long long t0, t1;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-        for (;;)
-        {
-            int v, h = hist_tick;
-            asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(ticks + HR_MAX_RANKS + lane) : "memory");
-            if (hist_tick > 0) asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(h) : "l"(ticks + lane) : "memory");
-            if (v >= rt_tick && h >= hist_tick) break;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-            if (t1 - t0 > 10000000000ull) { *err = 1 + lane; break; }
-            __nanosleep(100);
-        }
-    }
+    if (lane < world && lane != self && wait_tick(ticks + TICK_RT * HR_MAX_RANKS + lane, lane, rt_tick, err, 100))
+        wait_tick(ticks + TICK_HIST * HR_MAX_RANKS + lane, lane, hist_tick, err, 100); // ticks only grow: the same as one joint wait
     __syncwarp();
     const int          chunk = (MH + 31) / 32;
     unsigned long long local = 0;
@@ -353,27 +314,16 @@ __global__ void k_rt_wait_partition(const int* __restrict__ ticks, int rt_tick, 
 __global__ void k_peer_wait(const int* __restrict__ ticks, int world, int self, int tick, int* err)
 {
     const int r = threadIdx.x;
-    if (r >= world || r == self) return;
-    unsigned long long t0, t1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    for (;;)
-    {
-        int v;
-        asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(ticks + r) : "memory");
-        if (v >= tick) break;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-        if (t1 - t0 > 10000000000ull) { *err = 1 + r; break; } // a peer died or the ranks render different frame counts: do not hang the GPU
-        __nanosleep(200);
-    }
+    if (r < world && r != self) wait_tick(ticks + r, r, tick, err, 200);
 }
 
 // Interleaved cooperative ray trace (reflections, path tracer): block b copies this rank's chunk c = self + b * world (8 image rows of
 // RGBA16F texels) to every rank that reads those rows; the last block to finish publishes the ray-trace tick.  A rank that owns no
 // chunk still runs PUSH_SPLIT blocks so that its tick is published.
 #define PUSH_SPLIT 4
-struct RowPtrs { uint2* p[HR_MAX_RANKS]; };
 struct NeedRows { int r0[HR_MAX_RANKS], r1[HR_MAX_RANKS]; };
-__global__ void __launch_bounds__(256) k_rt_push_chunks(RowPtrs imgs, NeedRows need, TickPtrs ticks, int* __restrict__ ctl, int world, int self, int W, int H, int tick)
+__global__ void __launch_bounds__(256) k_rt_push_chunks(PeerPtrs<uint2> imgs, NeedRows need, PeerPtrs<int> ticks, int* __restrict__ ctl, int world, int self, int W, int H,
+                                                        int tick)
 {
     // PUSH_SPLIT blocks share one chunk (a chunk is 8 rows x W texels = 245 KB at 4K: one block would walk it in 60 dependent round trips)
     const int c = self + ((int)blockIdx.x / PUSH_SPLIT) * world, part = (int)blockIdx.x % PUSH_SPLIT, r0 = c * 8, r1 = min(r0 + 8, H);
@@ -388,37 +338,21 @@ __global__ void __launch_bounds__(256) k_rt_push_chunks(RowPtrs imgs, NeedRows n
             uint4*       d4 = reinterpret_cast<uint4*>(imgs.p[q] + first);
             for (size_t i = (size_t)part * blockDim.x + threadIdx.x; i < n / 2; i += (size_t)PUSH_SPLIT * blockDim.x) d4[i] = s4[i];
         }
-    __threadfence_system();
-    __syncthreads();
-    __shared__ int s_last;
-    if (threadIdx.x == 0)
-    {
-        const int done = atomicAdd(ctl + HR_MAX_RANKS + 2, 1);
-        s_last         = done == (int)gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!s_last) return;
-    if (threadIdx.x == 0) ctl[HR_MAX_RANKS + 2] = 0;
-    const int r = threadIdx.x;
-    if (r < world && r != self && ticks.p[r])
-    {
-        __threadfence_system();
-        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
-    }
+    publish_when_grid_done(ctl, ticks, world, self, TICK_RT, tick);
 }
 
-// The two count images of the cooperative spp > 1 trace (shared images 7-8, by frame parity): allocated when a shadows / AO pass is
+// The two count images of the cooperative spp > 1 trace (SHARED_COUNT, by frame parity): allocated when a shadows / AO pass is
 // linked, so only linked passes pay their 2 B per pass pixel (16.6 MB at 3840x2160, 66 MB at 7680x4320).  They exist before the
 // first render, so switching spp on linked ranks needs no further collective.
 int rt_alloc_counts(hr_pass* p)
 {
-    if (p->n_hist < 9 || p->count_pp[0]) return HR_OK;
+    if ((p->kind != PASS_SHADOWS && p->kind != PASS_AO) || p->count_pp[0]) return HR_OK;
     for (int k = 0; k < 2; k++)
     {
         HR_CUDA(p->ctx, cudaMalloc((void**)&p->count_pp[k], (size_t)p->W * p->H));
         p->allocs.push_back(p->count_pp[k]);
         HR_CUDA(p->ctx, cudaMemset(p->count_pp[k], 0, (size_t)p->W * p->H));
-        p->hist_local[7 + k] = p->count_pp[k];
+        p->hist_local[SHARED_COUNT + k] = p->count_pp[k];
     }
     return HR_OK;
 }
@@ -520,7 +454,7 @@ void hr_peer_hist(const hr_pass* p, int img_k, int aux_k, int H, bool no_history
     const hr_ctx* ctx = p->ctx;
     HistPeers     hp {};
     hp.no_history = no_history ? 1 : 0;
-    if (p->peers_linked && ctx->world > 1)
+    if (hr_peer_linked(p))
     {
         hp.world = ctx->world;
         hp.self  = ctx->rank;
@@ -544,47 +478,50 @@ void hr_peer_hist(const hr_pass* p, int img_k, int aux_k, int H, bool no_history
     *out = hp;
 }
 
-int hr_peer_wait(hr_pass* p, int which, int tick, cudaStream_t st)
+// The device address of the time-out flag of the wait kernels, or the error of an earlier wait that timed out.
+static int sync_error_ptr(hr_pass* p, int** d_err)
 {
-    if (!p->peers_linked || p->ctx->world <= 1 || tick <= 0) return HR_OK;
     hr_ctx* ctx = p->ctx;
     if (p->sync_error && *p->sync_error)
     {
-        hr_set_error(ctx, "peer history: timed out waiting for rank %d's frame tick (peer stopped, or ranks rendered different frame counts)", *p->sync_error - 1);
+        hr_set_error(ctx, "peer sync: timed out waiting for rank %d's frame tick (peer stopped, or ranks rendered different frame counts)", *p->sync_error - 1);
         return HR_ERR_NCCL;
     }
-    int* d_err = nullptr;
-    HR_CUDA(ctx, cudaHostGetDevicePointer((void**)&d_err, p->sync_error, 0));
-    k_peer_wait<<<1, 32, 0, st>>>(p->sync_ticks + which * HR_MAX_RANKS, ctx->world, ctx->rank, tick, d_err);
-    ctx->launches++;
+    HR_CUDA(ctx, cudaHostGetDevicePointer((void**)d_err, p->sync_error, 0));
     return HR_OK;
 }
 
-int hr_peer_signal(hr_pass* p, int which, int tick, cudaStream_t st)
+int hr_peer_wait(hr_pass* p, int slot, int tick, cudaStream_t st)
 {
-    if (!p->peers_linked || p->ctx->world <= 1) return HR_OK;
-    TickPtrs t {};
-    for (int r = 0; r < p->ctx->world; r++) t.p[r] = p->peer_ticks[r];
-    k_peer_signal<<<1, 32, 0, st>>>(t, p->ctx->world, p->ctx->rank, which, tick);
+    if (!hr_peer_linked(p) || tick <= 0) return HR_OK;
+    int* d_err = nullptr;
+    int  rc    = sync_error_ptr(p, &d_err);
+    if (rc != HR_OK) return rc;
+    k_peer_wait<<<1, 32, 0, st>>>(p->sync_ticks + slot * HR_MAX_RANKS, p->ctx->world, p->ctx->rank, tick, d_err);
+    p->ctx->launches++;
+    return HR_OK;
+}
+
+int hr_peer_signal(hr_pass* p, int slot, int tick, cudaStream_t st)
+{
+    if (!hr_peer_linked(p)) return HR_OK;
+    k_peer_signal<<<1, 32, 0, st>>>(peer_tick_ptrs(p), p->ctx->world, p->ctx->rank, slot, tick);
     p->ctx->launches++;
     return HR_OK;
 }
 
 int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* need1, cudaStream_t st)
 {
-    hr_ctx* ctx = p->ctx;
-    RowPtrs  im {};
+    hr_ctx*  ctx = p->ctx;
     NeedRows nd {};
-    TickPtrs t {};
     for (int r = 0; r < ctx->world; r++)
     {
-        im.p[r]  = static_cast<uint2*>(p->hist_peer[r][img]);
         nd.r0[r] = need0[r];
         nd.r1[r] = need1[r];
-        t.p[r]   = p->peer_ticks[r];
     }
     const int n_chunks = (p->H + 7) / 8, mine = (n_chunks - ctx->rank + ctx->world - 1) / ctx->world;
-    k_rt_push_chunks<<<(mine > 0 ? mine : 1) * PUSH_SPLIT, 256, 0, st>>>(im, nd, t, p->rt_bounds, ctx->world, ctx->rank, p->W, p->H, tick);
+    k_rt_push_chunks<<<(mine > 0 ? mine : 1) * PUSH_SPLIT, 256, 0, st>>>(peer_image_ptrs<uint2>(p, img), nd, peer_tick_ptrs(p), p->rt_bounds, ctx->world, ctx->rank,
+                                                                        p->W, p->H, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -593,15 +530,15 @@ int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* n
 // Linked DDGI passes split the probe stages by z-slices (hr_api_gi.inc).  The slices of a rank are one contiguous row range of each
 // atlas, which the rank stores into every peer's atlas of this frame's ping-pong after its K19/K20 (k_ddgi_push), so every rank
 // holds the complete atlases without a collective on the render stream.  The atlases are allocated when the grid is (re)initialised,
-// after the passes were linked, so the push reads the peers' addresses at run time from this rank's table (shared image 0,
+// after the passes were linked, so the push reads the peers' addresses at run time from this rank's table (SHARED_DDGI_TAB,
 // [rank][irradiance 0, irradiance 1, depth 0, depth 1]):
 //   * same-process ranks render one after another from one thread, so rank 0 enqueues the push of a re-initialisation frame before
 //     rank 1 has allocated its new atlases.  After a (re)initialisation every rank writes its addresses into its peers' tables on
-//     its stream and then publishes its ready tick (slot 1) = that render's frame tick (k_ddgi_publish); in that render the push
+//     its stream and then publishes its ready tick (TICK_DDGI_READY) = that render's frame tick (k_ddgi_publish); in that render the push
 //     is preceded by a one-warp wait until every peer's ready tick reached it (hr_api_gi.inc).
 //   * IPC ranks re-initialise in the same render (they render the same scene with the same parameters): they exchange the new
 //     atlases' IPC handles in a collective and write the mapped addresses into their own table; the push waits for nothing.
-// One frame tick (slot 0) orders the stores: a rank publishes tick N after its frame-N stores (last block of k_ddgi_push) and waits,
+// One frame tick (TICK_ATLAS) orders the stores: a rank publishes tick N after its frame-N stores (last block of k_ddgi_push) and waits,
 // before its K21, until every peer's tick reached N.
 //   * Write before read: K21 and the reflections of frame N read atlas[mp] after that wait, so it is complete.
 //   * Read before write: the frame-N stores go into atlas[mp], which a peer last read in frame N-1 (K18's infinite bounce, every
@@ -611,22 +548,20 @@ int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* n
 namespace {
 
 struct AtlasSet { void* a[4]; };
-struct TabPtrs { void** p[HR_MAX_RANKS]; };
-struct BytePtrs { uint8_t* const* p; };
 
-__global__ void k_ddgi_publish(TabPtrs tabs, TickPtrs ticks, AtlasSet mine, int world, int self, int tick)
+__global__ void k_ddgi_publish(PeerPtrs<void*> tabs, PeerPtrs<int> ticks, AtlasSet mine, int world, int self, int tick)
 {
     const int r = threadIdx.x;
     if (r >= world || r == self || !tabs.p[r] || !ticks.p[r]) return;
     for (int k = 0; k < 4; k++) tabs.p[r][self * 4 + k] = mine.a[k];
     __threadfence_system();
-    asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(ticks.p[r] + 1 * HR_MAX_RANKS + self), "r"(tick) : "memory");
+    st_release_sys(ticks.p[r] + TICK_DDGI_READY * HR_MAX_RANKS + self, tick);
 }
 
 // Bytes [i0, i1) of the irradiance atlas and [d0, d1) of the depth atlas (ping-pong mp) into every peer's atlas, at the addresses in
 // this rank's table; the last block publishes the atlas tick.
 __global__ void __launch_bounds__(256) k_ddgi_push(void* const* tab, const uint8_t* __restrict__ irr, const uint8_t* __restrict__ dep, size_t i0, size_t i1, size_t d0,
-                                                   size_t d1, int mp, TickPtrs peers, int* __restrict__ ctl, int world, int self, int tick)
+                                                   size_t d1, int mp, PeerPtrs<int> ticks, int* __restrict__ ctl, int world, int self, int tick)
 {
     __shared__ uint8_t* s_dst[2][HR_MAX_RANKS];
     const int r = threadIdx.x;
@@ -638,20 +573,9 @@ __global__ void __launch_bounds__(256) k_ddgi_push(void* const* tab, const uint8
     }
     __syncthreads();
     const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (size_t)gridDim.x * blockDim.x;
-    push_bytes(irr, BytePtrs { s_dst[0] }, world, self, i0, i1, tid, nthr);
-    push_bytes(dep, BytePtrs { s_dst[1] }, world, self, d0, d1, tid, nthr);
-    __threadfence_system();
-    __syncthreads();
-    __shared__ int s_last;
-    if (threadIdx.x == 0) s_last = atomicAdd(ctl + HR_MAX_RANKS + 2, 1) == (int)gridDim.x - 1;
-    __syncthreads();
-    if (!s_last) return;
-    if (threadIdx.x == 0) ctl[HR_MAX_RANKS + 2] = 0; // blocks-done counter
-    if (r < world && r != self && peers.p[r])
-    {
-        __threadfence_system(); // all blocks' stores (ordered before their atomicAdd) are visible before the tick
-        asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(peers.p[r] + self), "r"(tick) : "memory");
-    }
+    push_bytes(irr, s_dst[0], world, self, i0, i1, tid, nthr);
+    push_bytes(dep, s_dst[1], world, self, d0, d1, tid, nthr);
+    publish_when_grid_done(ctl, ticks, world, self, TICK_ATLAS, tick);
 }
 
 } // namespace
@@ -688,14 +612,7 @@ int hr_ddgi_publish(hr_pass* p, int tick, cudaStream_t st)
     }
     else
     {
-        TabPtrs  t {};
-        TickPtrs k {};
-        for (int r = 0; r < ctx->world; r++)
-        {
-            t.p[r] = static_cast<void**>(p->hist_peer[r][0]);
-            k.p[r] = p->peer_ticks[r];
-        }
-        k_ddgi_publish<<<1, 32, 0, st>>>(t, k, mine, ctx->world, ctx->rank, tick);
+        k_ddgi_publish<<<1, 32, 0, st>>>(peer_image_ptrs<void*>(p, SHARED_DDGI_TAB), peer_tick_ptrs(p), mine, ctx->world, ctx->rank, tick);
         ctx->launches++;
     }
     p->ddgi_ready = tick;
@@ -705,10 +622,8 @@ int hr_ddgi_publish(hr_pass* p, int tick, cudaStream_t st)
 int hr_ddgi_push(hr_pass* p, int mp, size_t i0, size_t i1, size_t d0, size_t d1, int tick, cudaStream_t st)
 {
     hr_ctx* ctx = p->ctx;
-    TickPtrs t {};
-    for (int r = 0; r < ctx->world; r++) t.p[r] = p->peer_ticks[r];
-    k_ddgi_push<<<ctx->sm_count, 256, 0, st>>>(p->ddgi_tab, (const uint8_t*)p->ddgi_irr[mp], (const uint8_t*)p->ddgi_depth[mp], i0, i1, d0, d1, mp, t, p->rt_bounds,
-                                               ctx->world, ctx->rank, tick);
+    k_ddgi_push<<<ctx->sm_count, 256, 0, st>>>(p->ddgi_tab, (const uint8_t*)p->ddgi_irr[mp], (const uint8_t*)p->ddgi_depth[mp], i0, i1, d0, d1, mp, peer_tick_ptrs(p),
+                                               p->rt_bounds, ctx->world, ctx->rank, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -727,9 +642,9 @@ static int rt_init_bounds(hr_pass* p)
 bool hr_rt_share(hr_pass* p, int parity, RtShare* out)
 {
     hr_ctx* ctx = p->ctx;
-    if (!p->peers_linked || ctx->world <= 1 || p->n_hist < 9) return false;
+    if (!hr_peer_linked(p) || (p->kind != PASS_SHADOWS && p->kind != PASS_AO)) return false;
     RtShare sh {};
-    sh.mask_local = static_cast<uint32_t*>(p->hist_local[4 + parity]);
+    sh.mask_local = static_cast<uint32_t*>(p->hist_local[SHARED_MASK + parity]);
     sh.bounds     = p->rt_bounds;
     sh.cost_acc   = p->rt_cost_acc;
     sh.world      = ctx->world;
@@ -741,21 +656,12 @@ bool hr_rt_share(hr_pass* p, int parity, RtShare* out)
 int hr_rt_share_finish(hr_pass* p, int parity, int tick, bool count, cudaStream_t st)
 {
     hr_ctx*   ctx = p->ctx;
-    const int MH = (p->H + 3) / 4, MW = (p->W + 7) / 8;
-    CostPtrs  c {};
-    MaskPtrs  m {};
-    CountPtrs n {};
-    TickPtrs  t {};
-    for (int r = 0; r < ctx->world; r++)
-    {
-        c.p[r] = static_cast<uint32_t*>(p->hist_peer[r][6]);
-        m.p[r] = static_cast<uint32_t*>(p->hist_peer[r][4 + parity]);
-        n.p[r] = static_cast<uint8_t*>(p->hist_peer[r][7 + parity]);
-        t.p[r] = p->peer_ticks[r];
-    }
-    // a count row holds 8x the bytes of a mask row: more blocks for the wider copy
-    if (count) k_rt_push_count<<<128, 256, 0, st>>>(n, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, p->W, p->H, tick);
-    else k_rt_push<<<32, 256, 0, st>>>(m, c, p->rt_bounds, p->rt_cost_acc, t, ctx->world, ctx->rank, parity, MH, MW, tick);
+    const int MH = (p->H + 3) / 4;
+    // mask row: one row of 4 * MW bytes; count image: 4 rows of W bytes, 8x the bytes of a mask row, so more blocks for the wider copy
+    const int    blocks = count ? 128 : 32, rows = count ? 4 : 1, height = count ? p->H : MH;
+    const size_t row_bytes = count ? (size_t)p->W : (size_t)4 * ((p->W + 7) / 8);
+    k_rt_push<<<blocks, 256, 0, st>>>(peer_image_ptrs<uint8_t>(p, (count ? SHARED_COUNT : SHARED_MASK) + parity), peer_image_ptrs<uint32_t>(p, SHARED_COST), p->rt_bounds,
+                                      p->rt_cost_acc, peer_tick_ptrs(p), ctx->world, ctx->rank, parity, MH, row_bytes, rows, height, tick);
     ctx->launches++;
     return HR_OK;
 }
@@ -764,13 +670,9 @@ int hr_rt_wait_partition(hr_pass* p, int parity, int rt_tick, int hist_tick, cud
 {
     hr_ctx*   ctx = p->ctx;
     const int MH  = (p->H + 3) / 4;
-    if (p->sync_error && *p->sync_error)
-    {
-        hr_set_error(ctx, "peer sync: timed out waiting for rank %d's frame tick (peer stopped, or ranks rendered different frame counts)", *p->sync_error - 1);
-        return HR_ERR_NCCL;
-    }
-    int* d_err = nullptr;
-    HR_CUDA(ctx, cudaHostGetDevicePointer((void**)&d_err, p->sync_error, 0));
+    int*      d_err = nullptr;
+    int       rc    = sync_error_ptr(p, &d_err);
+    if (rc != HR_OK) return rc;
     k_rt_wait_partition<<<1, 32, 0, st>>>(p->sync_ticks, rt_tick, hist_tick, d_err, p->rt_cost_all + (size_t)parity * MH, MH, ctx->world, ctx->rank,
                                          hr_rt_share_cap(MH, ctx->world), p->rt_bounds);
     ctx->launches++;

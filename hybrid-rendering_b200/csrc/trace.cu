@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(RT_CTA_WARPS * 32) k_ray_trace_mask_shared(GBu
     count_rays(fc.ray_ctr, 0, traced ? 1u : 0u);
 }
 
-// spp > 1 form of the cooperative trace: the share's pixels go to this rank's count image (k_rt_push_count copies them to the
+// spp > 1 form of the cooperative trace: the share's pixels go to this rank's count image (k_rt_push copies them to the
 // peers).  trace_pixel_spp is the function of k_ray_trace_count, so the counts equal the single-GPU counts bit for bit.  A warp's
 // duration grows about linearly with spp, so it is added to the row cost in units of 2^cost_shift cycles, cost_shift = 6 +
 // ceil(log2 spp): the row sums stay in the range of the 1-spp trace (scaling every row alike leaves the partition unchanged)

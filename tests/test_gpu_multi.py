@@ -25,7 +25,7 @@ SH = dict(temporal=1, atrous=2, moments=4, prev=5, final=100)
 AO = dict(temporal=1, blur=2, length=4, final=100)
 
 
-def frames(n, pan_from=3, vertical=0.0):
+def frames(n, pan_from=3, vertical=0.0, W=W, H=H):
     f = None
     for i in range(n):
         dx = 0.0 if i < pan_from else 0.05 * (i - pan_from + 1)
@@ -34,7 +34,7 @@ def frames(n, pan_from=3, vertical=0.0):
         yield f
 
 
-def make_rank(device, sc, sh_scale, ao_scale, rank=0, world=1):
+def make_rank(device, sc, sh_scale, ao_scale, rank=0, world=1, W=W, H=H):
     c = pyhr.Context(device)
     c.set_bluenoise(*pyhr.blue_noise())
     c.build_scene(sc)
@@ -83,11 +83,17 @@ def test_sharded_emulation_bit_identical(world, sh_scale, ao_scale):
         c.close()
 
 
-@pytest.mark.parametrize("world,sh_scale,ao_scale", [(2, 0, 1), (5, 0, 0), (8, 1, 1)])
-def test_peer_history_emulation_bit_identical(world, sh_scale, ao_scale):
+# 1366x768: mask rows of 684 bytes and count rows of 5464 bytes, neither a multiple of 16, so the peer pushes take their
+# 4-byte and byte-wise paths
+PEER_CASES = [pytest.param(w, s, a, W, H, id=f"{w}-{s}-{a}") for w, s, a in [(2, 0, 1), (5, 0, 0), (8, 1, 1)]]
+PEER_CASES += [pytest.param(w, 0, 0, 1366, 768, id=f"1366x768-{w}") for w in (3, 8)]
+
+
+@pytest.mark.parametrize("world,sh_scale,ao_scale,W,H", PEER_CASES)
+def test_peer_history_emulation_bit_identical(world, sh_scale, ao_scale, W, H):
     sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
-    ref = make_rank(0, sc, sh_scale, ao_scale)
-    ranks = [make_rank(0, sc, sh_scale, ao_scale, r, world) for r in range(world)]
+    ref = make_rank(0, sc, sh_scale, ao_scale, W=W, H=H)
+    ranks = [make_rank(0, sc, sh_scale, ao_scale, r, world, W, H) for r in range(world)]
     for r in range(world):
         for q in range(world):
             if q != r:
@@ -98,7 +104,7 @@ def test_peer_history_emulation_bit_identical(world, sh_scale, ao_scale):
     # cost-balanced share of the whole image and pushes it to all peers), so the emulated ranks must be able to run
     # concurrently: one CUDA stream per rank (conftest.py raises CUDA_DEVICE_MAX_CONNECTIONS so they get separate queues).
     streams = [torch.cuda.Stream() for _ in range(world)]
-    for f in frames(8, pan_from=2, vertical=0.35):
+    for f in frames(8, pan_from=2, vertical=0.35, W=W, H=H):
         g = pyhr.write_gbuffer(sc, f, W, H)
         ref[0].gbuffer_upload(f.ping_pong, g)
         ref[1].render(f)
@@ -311,7 +317,7 @@ def _nccl_ddgi_worker(rank, world, uid, result_dir):
 
 
 def test_nccl_sharded_ddgi_and_reflections_match_single(tmp_path):
-    """DDGI probe stages split by z-slices + atlas all-gather, per-pixel sampling by bands, half-res reflections reading the atlas:
+    """DDGI probe stages split by z-slices + atlas push to every peer, per-pixel sampling by bands, half-res reflections reading the atlas:
     atlases, DDGI sample and the reflections output are complete on every rank and equal the single-GPU images bit for bit."""
     import torch
     world = min(torch.cuda.device_count(), 8)
