@@ -89,6 +89,44 @@ __device__ __forceinline__ float2 rn_virtual_point_reprojection(int x, int y, fl
     return make_float2(__fmul_rn(__fadd_rn(__fmul_rn(rx, 0.5f), 0.5f), fw), __fmul_rn(__fadd_rn(__fmul_rn(ry, 0.5f), 0.5f), fh));
 }
 
+// ---- the reprojection's validity test, exactly rounded ----------------------------------------------------------------
+// is_reprojection_valid (reprojection.glsl:52-67) decides a pixel's history length and with it the tile flags, which the
+// oracle's statement fixes bit for bit: a plane distance or a normal dot^2 within ulps of PLANE_DISTANCE / NORMAL_DISTANCE
+// flips with one rounding.  Positions, normals and dots are therefore rounded as oracle/orc_glsl.h rounds them: (x*x' + y*y') +
+// z*z', normalize = v * (1 / sqrt(v.v)), world position = (M * (2u - 1, 2v - 1, d, 1)).xyz / w, tex coord = (x + 0.5) / W.
+__device__ __forceinline__ float rn_dot3(float3 a, float3 b) { return __fadd_rn(__fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fmul_rn(a.z, b.z)); }
+__device__ __forceinline__ float3 rn_octohedral_to_direction(float ex, float ey) // common.glsl:150-156
+{
+    float x = ex, y = ey;
+    const float z = __fsub_rn(__fsub_rn(1.0f, fabsf(ex)), fabsf(ey));
+    if (z < 0.0f)
+    {
+        x = __fsub_rn(1.0f, fabsf(ey)) * (ex < 0.0f ? -1.0f : 1.0f);
+        y = __fsub_rn(1.0f, fabsf(ex)) * (ey < 0.0f ? -1.0f : 1.0f);
+    }
+    const float3 v   = make_float3(x, y, z);
+    const float  inv = __fdiv_rn(1.0f, __fsqrt_rn(rn_dot3(v, v)));
+    return make_float3(__fmul_rn(x, inv), __fmul_rn(y, inv), __fmul_rn(z, inv));
+}
+__device__ __forceinline__ float3 rn_world_position_from_depth(float u, float v, float d, const float* __restrict__ M) // common.glsl:169-184
+{
+    const float4 w = rn_mat_point(M, rn_mad(u, 2.0f, -1.0f), rn_mad(v, 2.0f, -1.0f), d);
+    return make_float3(__fdiv_rn(w.x, w.w), __fdiv_rn(w.y, w.w), __fdiv_rn(w.z, w.w));
+}
+// a history texel as the validity test reads it: octahedral normal, mesh id, depth (all zero out of bounds, like texelFetch)
+struct HistTap { float ex, ey, mesh_id, depth; };
+// is_reprojection_valid minus the frame test, which the callers hoist.  cur_pos / cur_n: rn_world_position_from_depth /
+// rn_octohedral_to_direction of the pixel; (hu, hv): its history tex coord, tex coord + motion rounded once
+__device__ __forceinline__ bool rn_tap_valid(const HistTap& t, float3 cur_pos, float3 cur_n, float cur_mesh, float hu, float hv, const float* __restrict__ vpi)
+{
+    if (!(cur_mesh == t.mesh_id)) return false;
+    const float3 hp = rn_world_position_from_depth(hu, hv, t.depth, vpi);
+    const float3 d  = make_float3(__fsub_rn(cur_pos.x, hp.x), __fsub_rn(cur_pos.y, hp.y), __fsub_rn(cur_pos.z, hp.z));
+    if (fabsf(rn_dot3(d, cur_n)) > 5.0f) return false; // PLANE_DISTANCE
+    const float nd = fabsf(rn_dot3(cur_n, rn_octohedral_to_direction(t.ex, t.ey)));
+    return __fmul_rn(nd, nd) > 0.1f;                     // NORMAL_DISTANCE
+}
+
 // common.glsl:169-184
 __device__ __forceinline__ float3 world_position_from_depth(float u, float v, float d, const float* __restrict__ M)
 {

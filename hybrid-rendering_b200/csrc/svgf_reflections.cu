@@ -14,30 +14,17 @@ __device__ __forceinline__ bool inside(int x, int y, int W, int H) { return x >=
 __device__ __forceinline__ float luminance(float r, float g, float b) { return fmaxf(r * 0.299f + g * 0.587f + b * 0.114f, 0.0001f); }
 __device__ __forceinline__ uint2 pack_h4(float a, float b, float c, float d) { return make_uint2(f2_to_h2(a, b), f2_to_h2(c, d)); }
 
-struct Tap { float3 n; float mesh_id; float depth; };
-__device__ __forceinline__ Tap fetch_prev(const GBufLevelDev& p, int x, int y)
+__device__ __forceinline__ HistTap fetch_prev(const GBufLevelDev& p, int x, int y)
 {
-    Tap t;
+    HistTap t { 0.0f, 0.0f, 0.0f, 0.0f }; // texelFetch out of bounds => zeros
     if (inside(x, y, p.W, p.H))
     {
         const size_t i  = (size_t)y * p.W + x;
         const float2 e  = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(p.gb2 + i)));
         const float2 g3 = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(p.gb3 + i) + 1));
-        t.n = octohedral_to_direction(e.x, e.y);
-        t.mesh_id = g3.x;
-        t.depth   = __ldg(p.depth + i);
+        t = HistTap { e.x, e.y, g3.x, __ldg(p.depth + i) };
     }
-    else { t.n = octohedral_to_direction(0.0f, 0.0f); t.mesh_id = 0.0f; t.depth = 0.0f; }
     return t;
-}
-__device__ __forceinline__ bool tap_valid(const Tap& t, float3 cur_pos, float3 cur_n, float cur_mesh, float hu, float hv, const float* vpi)
-{
-    if (!(cur_mesh == t.mesh_id)) return false;
-    const float3 hp = world_position_from_depth(hu, hv, t.depth, vpi);
-    const float3 d  = make_float3(cur_pos.x - hp.x, cur_pos.y - hp.y, cur_pos.z - hp.z);
-    if (fabsf(dot3(d, cur_n)) > 5.0f) return false;
-    const float nd = fabsf(dot3(cur_n, t.n));
-    return nd * nd > 0.1f;
 }
 
 struct ReflTemporalParams { float alpha, moments_alpha; int approximate_with_ddgi; int row0, row1; int rot; }; // rot: the last `rot` tile rows are scheduled first
@@ -165,9 +152,9 @@ __global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBuf
             const float ray_length = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(input + idx) + 1)).y;
             const float fw = (float)W, fh = (float)H;
             const float tu = ((float)x + 0.5f) / fw, tv = ((float)y + 0.5f) / fh;
-            const float3 cn = octohedral_to_direction(g2.x, g2.y);
+            const float3 cn = rn_octohedral_to_direction(g2.x, g2.y);
             const float  cmesh = g3.z, curvature = g3.y;
-            const float3 cpos = world_position_from_depth(tu, tv, depth, fc.view_proj_inverse);
+            const float3 cpos = rn_world_position_from_depth(tu, tv, depth, fc.view_proj_inverse);
             // compute_history_coord, reprojection.glsl:101-111
             float hfx = rn_mad(g2.z, fw, (float)x), hfy = rn_mad(g2.w, fh, (float)y);
             if (ray_length > 0.0f && curvature == 0.0f)
@@ -177,7 +164,7 @@ __global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBuf
                 hfy = vp.y;
             }
             const int   hcx = (int)hfx, hcy = (int)hfy; // ivec2(reprojected_coord) :171
-            const float hu = tu + g2.z, hv = tv + g2.w;
+            const float hu = __fadd_rn(tu, g2.z), hv = __fadd_rn(tv, g2.w);
             const bool  in_frame = inside(hcx, hcy, W, H);
             const OwnerCache oc = owner_cache<PEER>(hp, max(hcy - 1, 0), min(hcy + 1, H - 1));
             float hc[3] = { 0, 0, 0 }, hm0 = 0.0f, hm1 = 0.0f;
@@ -193,8 +180,8 @@ __global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBuf
                 {
                     if (w4[s] == 0.0f) continue; // exact: see svgf_temporal.cu
                     const int px = hcx + (s & 1), py = hcy + (s >> 1);
-                    const Tap t  = fetch_prev(prev, px, py);
-                    if (tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                    const HistTap t = fetch_prev(prev, px, py);
+                    if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                     {
                         any = true;
                         if (inside(px, py, W, H))
@@ -221,8 +208,8 @@ __global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBuf
                         for (int xx = -1; xx <= 1; xx++)
                         {
                             const int px = hcx + xx, py = hcy + yy;
-                            const Tap t  = fetch_prev(prev, px, py);
-                            if (tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                            const HistTap t = fetch_prev(prev, px, py);
+                            if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                             {
                                 if (inside(px, py, W, H))
                                 {

@@ -14,27 +14,17 @@ namespace {
 
 using namespace gf;
 
-struct Tap { float3 n; float mesh_id; float depth; };
-
 __device__ __forceinline__ bool inside(int x, int y, int W, int H) { return x >= 0 && y >= 0 && x < W && y < H; }
 
-__device__ __forceinline__ Tap fetch_prev(const GBufLevelDev& p, int x, int y)
+__device__ __forceinline__ HistTap fetch_prev(const GBufLevelDev& p, int x, int y)
 {
-    Tap t;
+    HistTap t { 0.0f, 0.0f, 0.0f, 0.0f }; // texelFetch out of bounds => zeros
     if (inside(x, y, p.W, p.H))
     {
         const size_t i  = (size_t)y * p.W + x;
         const float2 e  = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(p.gb2 + i)));
         const float2 g3 = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(p.gb3 + i) + 1)); // (mesh id, linear z)
-        t.n       = octohedral_to_direction(e.x, e.y);
-        t.mesh_id = g3.x;
-        t.depth   = __ldg(p.depth + i);
-    }
-    else
-    { // texelFetch out of bounds => zeros
-        t.n       = octohedral_to_direction(0.0f, 0.0f);
-        t.mesh_id = 0.0f;
-        t.depth   = 0.0f;
+        t = HistTap { e.x, e.y, g3.x, __ldg(p.depth + i) };
     }
     return t;
 }
@@ -50,38 +40,10 @@ __device__ __forceinline__ TapRaw fetch_prev_raw(const GBufLevelDev& p, size_t i
     return r;
 }
 
-__device__ __forceinline__ Tap decode_tap(const TapRaw& r)
+__device__ __forceinline__ HistTap decode_tap(const TapRaw& r)
 { // all-zero words decode to the out-of-bounds texel: normal oct(0,0), mesh id 0, depth 0
-    Tap          t;
     const float2 e = h2_to_f2(r.e);
-    t.n       = octohedral_to_direction(e.x, e.y);
-    t.mesh_id = h2_to_f2(r.g3).x;
-    t.depth   = r.depth;
-    return t;
-}
-
-// world_position_from_depth (common.glsl:175-186) with an approximate reciprocal: only feeds the 5.0-unit plane-distance test
-__device__ __forceinline__ float3 world_position_from_depth_fast(float u, float v, float d, const float* __restrict__ M)
-{
-    const float sx = u * 2.0f - 1.0f, sy = v * 2.0f - 1.0f;
-    const float wx = M[0] * sx + M[4] * sy + M[8] * d + M[12];
-    const float wy = M[1] * sx + M[5] * sy + M[9] * d + M[13];
-    const float wz = M[2] * sx + M[6] * sy + M[10] * d + M[14];
-    const float ww = M[3] * sx + M[7] * sy + M[11] * d + M[15];
-    const float iw = fast_rcp(ww);
-    return make_float3(wx * iw, wy * iw, wz * iw);
-}
-
-// is_reprojection_valid, reprojection.glsl:52-67 (frame test hoisted by the caller)
-__device__ __forceinline__ bool tap_valid(const Tap& t, float3 cur_pos, float3 cur_n, float cur_mesh, float hu, float hv, const float* vpi)
-{
-    if (!(cur_mesh == t.mesh_id)) return false;
-    const float3 hp = world_position_from_depth_fast(hu, hv, t.depth, vpi);
-    const float3 d  = make_float3(cur_pos.x - hp.x, cur_pos.y - hp.y, cur_pos.z - hp.z);
-    if (fabsf(dot3(d, cur_n)) > 5.0f) return false; // PLANE_DISTANCE
-    const float nd = fabsf(dot3(cur_n, t.n));
-    if (!(nd * nd > 0.1f)) return false; // NORMAL_DISTANCE
-    return true;
+    return HistTap { e.x, e.y, h2_to_f2(r.g3).x, r.depth };
 }
 
 // ---- history fetches through the owner table (HistPeers, hr_internal.h) ----
@@ -173,12 +135,12 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
             const float vis = (float)((s_rows[ly + 8] >> (lx + 8)) & 1ull);
             // ---- reproject(), reprojection.glsl:115-328 ----
             const float  fw = (float)W, fh = (float)H;
-            const float  tu = ((float)x + 0.5f) * fast_rcp(fw), tv = ((float)y + 0.5f) * fast_rcp(fh);
+            const float  tu = __fdiv_rn((float)x + 0.5f, fw), tv = __fdiv_rn((float)y + 0.5f, fh); // tex_coord, rounded as the validity test needs it
             const float4 g2 = h4_to_f4(g2raw);
             const float  cmesh = h2_to_f2(g3raw).x;
             const float  hfx = rn_mad(g2.z, fw, (float)x), hfy = rn_mad(g2.w, fh, (float)y); // history_coord_floor (:176), exactly rounded
             const int    hcx = (int)__fadd_rn(hfx, 0.5f), hcy = (int)__fadd_rn(hfy, 0.5f);       // history_coord (:175)
-            const float  hu = tu + g2.z, hv = tv + g2.w;                           // history_tex_coord (:177)
+            const float  hu = __fadd_rn(tu, g2.z), hv = __fadd_rn(tv, g2.w);       // history_tex_coord (:177)
             const bool   in_frame = inside(hcx, hcy, W, H);                        // out_of_frame_disocclusion_check on history_coord
             const int    bx = (int)hfx, by = (int)hfy;                             // ivec2(history_coord_floor) truncates
 
@@ -219,15 +181,15 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
                         else hraw[s] = hist_ld16<PEER>(hp.img, hp, py, pi);
                     }
                 }
-                const float3 cn   = octohedral_to_direction(g2.x, g2.y);
-                const float3 cpos = world_position_from_depth_fast(tu, tv, depth, fc.view_proj_inverse);
+                const float3 cn   = rn_octohedral_to_direction(g2.x, g2.y);
+                const float3 cpos = rn_world_position_from_depth(tu, tv, depth, fc.view_proj_inverse);
                 float sumw = 0.0f;
                 bool  any  = false;
 #pragma unroll
                 for (int s = 0; s < 4; s++)
                 {
                     if (w4[s] == 0.0f) continue;
-                    if (tap_valid(decode_tap(tr[s]), cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                    if (rn_tap_valid(decode_tap(tr[s]), cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                     {
                         any = true;
                         const float2 hh = h2_to_f2(hraw[s]), mm = h2_to_f2(mraw[s]);
@@ -250,8 +212,8 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
                         for (int xx = -1; xx <= 1; xx++)
                         {
                             const int px = hcx + xx, py = hcy + yy;
-                            const Tap t  = fetch_prev(prev, px, py);
-                            if (tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                            const HistTap t = fetch_prev(prev, px, py);
+                            if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                             {
                                 if (inside(px, py, W, H))
                                 {
@@ -394,12 +356,12 @@ __device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev pr
             const float vis = __fdiv_rn((float)s_cnt[ly + 8][lx + 8], (float)spp);
             // ---- reproject(), reprojection.glsl:115-328 ----
             const float  fw = (float)W, fh = (float)H;
-            const float  tu = ((float)x + 0.5f) * fast_rcp(fw), tv = ((float)y + 0.5f) * fast_rcp(fh);
+            const float  tu = __fdiv_rn((float)x + 0.5f, fw), tv = __fdiv_rn((float)y + 0.5f, fh); // tex_coord, rounded as the validity test needs it
             const float4 g2 = h4_to_f4(g2raw);
             const float  cmesh = h2_to_f2(g3raw).x;
             const float  hfx = rn_mad(g2.z, fw, (float)x), hfy = rn_mad(g2.w, fh, (float)y); // history_coord_floor (:176), exactly rounded
             const int    hcx = (int)__fadd_rn(hfx, 0.5f), hcy = (int)__fadd_rn(hfy, 0.5f);       // history_coord (:175)
-            const float  hu = tu + g2.z, hv = tv + g2.w;                           // history_tex_coord (:177)
+            const float  hu = __fadd_rn(tu, g2.z), hv = __fadd_rn(tv, g2.w);       // history_tex_coord (:177)
             const bool   in_frame = inside(hcx, hcy, W, H);                        // out_of_frame_disocclusion_check on history_coord
             const int    bx = (int)hfx, by = (int)hfy;                             // ivec2(history_coord_floor) truncates
 
@@ -440,15 +402,15 @@ __device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev pr
                         else hraw[s] = hist_ld16<PEER>(hp.img, hp, py, pi);
                     }
                 }
-                const float3 cn   = octohedral_to_direction(g2.x, g2.y);
-                const float3 cpos = world_position_from_depth_fast(tu, tv, depth, fc.view_proj_inverse);
+                const float3 cn   = rn_octohedral_to_direction(g2.x, g2.y);
+                const float3 cpos = rn_world_position_from_depth(tu, tv, depth, fc.view_proj_inverse);
                 float sumw = 0.0f;
                 bool  any  = false;
 #pragma unroll
                 for (int s = 0; s < 4; s++)
                 {
                     if (w4[s] == 0.0f) continue;
-                    if (tap_valid(decode_tap(tr[s]), cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                    if (rn_tap_valid(decode_tap(tr[s]), cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                     {
                         any = true;
                         const float2 hh = h2_to_f2(hraw[s]), mm = h2_to_f2(mraw[s]);
@@ -471,8 +433,8 @@ __device__ __forceinline__ void temporal_count(GBufLevelDev cur, GBufLevelDev pr
                         for (int xx = -1; xx <= 1; xx++)
                         {
                             const int px = hcx + xx, py = hcy + yy;
-                            const Tap t  = fetch_prev(prev, px, py);
-                            if (tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                            const HistTap t = fetch_prev(prev, px, py);
+                            if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
                             {
                                 if (inside(px, py, W, H))
                                 {

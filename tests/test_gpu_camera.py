@@ -75,7 +75,8 @@ def _first(case, i):
 
 # ---------------------------------------------------------------------------------------------- shadows + AO
 def _sh_ao_isolated(case, reach):
-    """before / after hooks: the cut's history reset, then every stage of both chains fed the device's own inputs"""
+    """before / after hooks: the cut's history reset, then every stage of both chains fed the device's own inputs (the previous
+    frame's, or what after.hist holds: a planted history)"""
     hist = {}
 
     def before(i, f, passes, oracles):
@@ -92,7 +93,7 @@ def _sh_ao_isolated(case, reach):
         # ---- shadows temporal (K3), fed the device's feedback image and moments of the previous frame
         gc, gp = cur_g.c(osh.scale), prev_g.c(osh.scale)
         shw, shh = osh.W, osh.H
-        prev_img, prev_mom = hist["sh"] if not _first(case, i) else (np.zeros((shh, shw, 2), np.uint16), np.zeros((shh, shw, 4), np.uint16))
+        prev_img, prev_mom = hist["sh"] if "sh" in hist and i not in case.resets else (np.zeros((shh, shw, 2), np.uint16), np.zeros((shh, shw, 4), np.uint16))
         t, m, tf = np.zeros((shh, shw, 2), np.uint16), np.zeros((shh, shw, 4), np.uint16), np.zeros_like(osh.tile_flags)
         with reach.codes("K3", i, shw, shh):
             L.orc_shadows_temporal(C.byref(gc), C.byref(gp), P(np.ascontiguousarray(sh.download(0))), P(prev_img), P(prev_mom), C.byref(f), osh.params.alpha,
@@ -113,7 +114,7 @@ def _sh_ao_isolated(case, reach):
         # ---- AO temporal (K9), fed the device's colour and length of the previous frame
         gc, gp = cur_g.c(oao.scale), prev_g.c(oao.scale)
         aw, ah = oao.W, oao.H
-        prev_c, prev_l = hist["ao"] if not _first(case, i) else (np.zeros((ah, aw), np.uint16), np.zeros((ah, aw), np.uint16))
+        prev_c, prev_l = hist["ao"] if "ao" in hist and i not in case.resets else (np.zeros((ah, aw), np.uint16), np.zeros((ah, aw), np.uint16))
         col, ln, tf = np.zeros((ah, aw), np.uint16), np.zeros((ah, aw), np.uint16), np.zeros_like(oao.tile_flags)
         with reach.codes("K9", i, aw, ah):
             L.orc_ao_temporal(C.byref(gc), C.byref(gp), P(np.ascontiguousarray(ao.download(0))), P(prev_c), P(prev_l), C.byref(f), oao.params.alpha, P(col), P(ln), P(tf))
@@ -127,11 +128,12 @@ def _sh_ao_isolated(case, reach):
         L.orc_ao_bilateral_blur(C.byref(gc), P(dev_t), P(dev_tf), P(zbp), 1, 0, oao.params.blur_radius, P(b0))
         L.orc_ao_bilateral_blur(C.byref(gc), P(b0), P(dev_tf), P(zbp), 0, 1, oao.params.blur_radius, P(b1))
         _bounded(f16(ao.download(2)), O.h2f(b1), f"frame {i}: isolated AO blur", 1e-3, 4e-3)
-        up = np.zeros((H, W), np.uint16)
+        up = np.zeros((oao.H0, oao.W0), np.uint16)
         L.orc_upsample_scalar(C.byref(cur_g.c(0)), C.byref(gc), P(np.ascontiguousarray(ao.download(2))), 1, 1.0, oao.params.power, P(up))
         _bounded(f16(ao.download(100)), O.h2f(up), f"frame {i}: isolated AO upsample", 1e-3, 4e-3)
         hist["ao"] = (np.ascontiguousarray(ao.download(1)), np.ascontiguousarray(ao.download(4)))
 
+    after.hist = hist  # the history the isolated stages read next: {"sh" | "ao" | "rf": (image, aux)}; absent on a first frame
     return before, after
 
 
@@ -165,7 +167,7 @@ def _refl_isolated(case, reach):
         rw, rh = orf.W, orf.H
         first = _first(case, i)
         z = np.zeros((rh, rw, 4), np.uint16)
-        prev_t, prev_m = hist["rf"] if not first else (z, z)
+        prev_t, prev_m = hist["rf"] if "rf" in hist and i not in case.resets else (z, z)
         approx = 1 if (Q.approximate_with_ddgi and dd is not None and not first) else 0
         t, m, tf = np.zeros_like(z), np.zeros_like(z), np.zeros_like(orf.tile_flags)
         with reach.codes("K14", i, rw, rh):
@@ -184,6 +186,7 @@ def _refl_isolated(case, reach):
         close(f16(rf.download(2)), O.h2f(src), f"frame {i} isolated reflections a-trous")
         hist["rf"] = (np.ascontiguousarray(rf.download(1)), np.ascontiguousarray(rf.download(4)))
 
+    after.hist = hist  # the history the isolated stages read next: {"sh" | "ao" | "rf": (image, aux)}; absent on a first frame
     return before, after
 
 

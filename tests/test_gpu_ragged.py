@@ -96,6 +96,14 @@ def set_params(dst_list, params):
             setattr(P, k, v)
 
 
+def gbuffer_in(ctx, ss, i, f, W, H, gbuf):
+    """frame i's G-buffer into slot f.ping_pong: the device producer's (and the oracle's statement of it), or gbuf(i, f, ctx)'s"""
+    if gbuf is not None:
+        return gbuf(i, f, ctx)
+    ctx.gbuffer_render(f.ping_pong, f)
+    return O.gbuffer_render(ss, f, W, H)
+
+
 # ---------------------------------------------------------------------------------------------- shadows + AO
 def measure_sh_ao(w, sh, ao, osh, oao):
     w.add("sh temporal", f16(sh.download(1)), O.h2f(osh.temporal))
@@ -108,9 +116,11 @@ def measure_sh_ao(w, sh, ao, osh, oao):
 
 
 def run_shadows_ao(case, W, H, sh_scale, ao_scale, sh_params=None, ao_params=None, n=5, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0,
-                   cam=CAM_SHADOWS_TEST, light=None, check=check_all, pan_from=3, seq=None, before=None, after=None):
+                   cam=CAM_SHADOWS_TEST, light=None, check=check_all, pan_from=3, seq=None, before=None, after=None, gbuf=None, prev_gbuf=None):
     """seq: the (i, frame) sequence to run in place of frames(W, H, n, pan_from, vertical, cam, light); before(i, f, (sh, ao), (osh, oao))
-    runs before frame i's renders (a history reset), after(i, f, cur_g, prev_g, (sh, ao), (osh, oao)) after its comparisons"""
+    runs before frame i's renders (a history reset), after(i, f, cur_g, prev_g, (sh, ao), (osh, oao)) after its comparisons;
+    gbuf(i, f, ctx) -> GBufferHost: frame i's G-buffer, which the callable has put into slot f.ping_pong, in place of the producer's;
+    prev_gbuf: a GBufferHost uploaded as the G-buffer that precedes the first frame (else the slot holds zeros)"""
     sc = pyhr.SynthScene(scene, tris)
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
@@ -122,10 +132,12 @@ def run_shadows_ao(case, W, H, sh_scale, ao_scale, sh_params=None, ao_params=Non
     w = Worst(case)
     prev_g = O.zero_gbuf_mips(W, H)
     for i, f in (seq if seq is not None else frames(W, H, n, pan_from, vertical, cam, light)):
+        if i == 0 and prev_gbuf is not None:
+            ctx.gbuffer_upload(1 - f.ping_pong, prev_gbuf)
+            prev_g = O.GBufMips(prev_gbuf)
         if before:
             before(i, f, (sh, ao), (osh, oao))
-        ctx.gbuffer_render(f.ping_pong, f)
-        g = O.gbuffer_render(ss, f, W, H)
+        g = gbuffer_in(ctx, ss, i, f, W, H, gbuf)
         cur_g = O.GBufMips(g)
         same_gbuffer(ctx, f, cur_g, W, H, g.gb1)
         sh.render(f)
@@ -202,7 +214,8 @@ def check_ddgi(i, dd, odd, w, cmp=close):
 
 
 def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vertical=0.0, scene=pyhr.SCENE_SHADOWS_TEST, tris=0, cam=CAM_SHADOWS_TEST,
-                light=None, ddgi_params=None, lut=None, ddgi_hook=None, frame_hook=None, cmp=close, seq=None, before=None, after=None):
+                light=None, ddgi_params=None, lut=None, ddgi_hook=None, frame_hook=None, cmp=close, seq=None, before=None, after=None, gbuf=None,
+                prev_gbuf=None):
     """test_gpu_gi_refl.run at any size and scale (DDGI sampled at the reflections' scale), fed by the device G-buffer producer.
     ddgi_params: overrides of the DDGI parameter block; lut: a BRDF LUT set on the context and the oracle (the reflections' IBL
     specular term, as in test_deferred); ddgi_hook(i, f, rot, dd, odd, fresh) runs before frame i's DDGI render and returns the
@@ -210,7 +223,7 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
     after frame i's comparisons.  cmp: the comparison of the DDGI and reflections images (`close`, or a rule with its signature; a
     rule that sets cmp.stopped ends the run after the comparison that set it).
     scene: a SynthScene kind, or an object with SynthScene's interface.  seq, before(i, f, (dd, rf), (odd, orf)) and
-    after(i, f, cur_g, prev_g, (dd, rf), (odd, orf)): as in run_shadows_ao (after runs once the denoised images are compared)"""
+    after(i, f, cur_g, prev_g, (dd, rf), (odd, orf)), gbuf, prev_gbuf: as in run_shadows_ao (after runs once the denoised images are compared)"""
     sc = pyhr.SynthScene(scene, tris) if isinstance(scene, int) else scene
     ss = O.ShadingScene(sc, brute=sc.n_tris <= 4096)
     bn = pyhr.blue_noise()
@@ -238,10 +251,12 @@ def run_gi_refl(case, W, H, scale, with_ddgi, params=None, n=5, pan_from=3, vert
     w = Worst(case)
     prev_g = O.zero_gbuf_mips(W, H)
     for i, f in (seq if seq is not None else frames(W, H, n, pan_from, vertical, cam, light)):
+        if i == 0 and prev_gbuf is not None:
+            ctx.gbuffer_upload(1 - f.ping_pong, prev_gbuf)
+            prev_g = O.GBufMips(prev_gbuf)
         if before:
             before(i, f, (dd, rf), (odd, orf))
-        ctx.gbuffer_render(f.ping_pong, f)
-        g = O.gbuffer_render(ss, f, W, H)
+        g = gbuffer_in(ctx, ss, i, f, W, H, gbuf)
         cur_g = O.GBufMips(g)
         same_gbuffer(ctx, f, cur_g, W, H, g.gb1)
         if dd:
