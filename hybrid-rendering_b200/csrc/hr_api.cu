@@ -818,8 +818,8 @@ static int frame_begin(hr_pass* p, const hr_frame* f, bool denoise, const HaloPl
     fr->rt_halo     = h.ray_trace;
     fr->up0         = fr->b0 << p->scale;
     fr->up1         = fr->b1 >= p->H ? p->H0 : (fr->b1 << p->scale);
-    p->last_rows[0] = fr->row0;
-    p->last_rows[1] = fr->row1;
+    p->last_rows[0] = denoise ? fr->row0 : 0; // the tile statistics cover the rows the denoise stages ran on: none without them
+    p->last_rows[1] = denoise ? fr->row1 : 0;
     timer_begin(p, st);
     int rc = hr_peer_link_ipc(p, st); // first sharded render: map the peers' history / ray-trace images (collective, shard.cu)
     if (rc != HR_OK) return rc;
@@ -1296,11 +1296,10 @@ int hr_pass_output_checksum(hr_pass* p, int which, int row0, int row1, uint64_t*
     HR_REQUIRE(ctx, row0 >= 0 && row1 >= row0 && row1 <= img.height, HR_ERR_INVALID_ARG, "hr_pass_output_checksum: bad row range");
     cudaStream_t st = (cudaStream_t)stream;
     hr_wait_exchange(p, st);
-    const size_t row_bytes = (size_t)img.width * texel_size(img.format);
     unsigned long long* d = nullptr;
     HR_CUDA(ctx, cudaMalloc((void**)&d, sizeof(unsigned long long)));
     HR_CUDA(ctx, cudaMemsetAsync(d, 0, sizeof(unsigned long long), st));
-    launch_checksum(img.data, row_bytes * row0, row_bytes * row1, d, st);
+    launch_checksum(img.data, texel_size(img.format), (size_t)img.width * row0, (size_t)img.width * row1, d, st);
     unsigned long long h = 0;
     cudaError_t e = cudaMemcpyAsync(&h, d, sizeof(h), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
@@ -1334,6 +1333,8 @@ int hr_pass_stage_times(hr_pass* p, const char** names, float* ms, int cap, int*
     *n = 0;
     StageTimer& T = p->timer;
     if (T.recs.empty()) return HR_OK;
+    // by name: the stage list changes between renders (a first TAA render's reset blit, filter_iterations, the gather, the upsample),
+    // so each name's entry is the mean over the renders that recorded it, in first-seen order
     std::vector<double> sum;
     std::vector<int>    cnt;
     T.last_names.clear();
@@ -1344,9 +1345,11 @@ int hr_pass_stage_times(hr_pass* p, const char** names, float* ms, int cap, int*
         {
             float t = 0.0f;
             cudaEventElapsedTime(&t, r.ev[i], r.ev[i + 1]);
-            if (i >= sum.size()) { sum.push_back(0.0); cnt.push_back(0); T.last_names.push_back(r.names[i]); }
-            sum[i] += t;
-            cnt[i]++;
+            size_t j = 0;
+            while (j < T.last_names.size() && T.last_names[j] != r.names[i]) j++;
+            if (j == T.last_names.size()) { sum.push_back(0.0); cnt.push_back(0); T.last_names.push_back(r.names[i]); }
+            sum[j] += t;
+            cnt[j]++;
         }
         for (auto e : r.ev) T.pool.push_back(e);
     }

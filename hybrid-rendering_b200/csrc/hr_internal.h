@@ -372,7 +372,7 @@ void launch_tonemap(const void* src, int channels, int W, int H, float exposure,
 // stats.cu (measurement helpers, not on the frame path)
 void launch_tile_stats(const uint8_t* flags, int TW, int t0, int t1, unsigned long long* d_out, cudaStream_t st);
 void launch_drain_ray_counters(unsigned long long* ctr, unsigned long long* d_out, cudaStream_t st);
-void launch_checksum(const void* base, size_t byte0, size_t byte1, unsigned long long* d_out, cudaStream_t st);
+void launch_checksum(const void* base, int texel_bytes, size_t texel0, size_t texel1, unsigned long long* d_out, cudaStream_t st);
 int hr_launch_build_mips(hr_ctx* ctx, GBufSlot& s, int W, int H, cudaStream_t st);
 int hr_bvh_build(hr_scene* sc, cudaStream_t st);
 BvhDev hr_bvh_view(const hr_scene* sc);

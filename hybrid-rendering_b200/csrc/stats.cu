@@ -3,8 +3,9 @@
 //     computes the a-trous roofline on the bytes the launch really processed (SURVEY.md §8d; the reference's K2/K4 tile lists
 //     `ray_traced_shadows.cpp:224` are this flag image here);
 //   * ray counters: drained from the per-pass counter slots the trace kernels add to (traverse.cuh::count_rays);
-//   * image checksum: order-independent 64-bit sum of mix(index, value) over the texels of an output — lets a sharded run prove
-//     on the device that its gathered frame equals the single-GPU frame.
+//   * image checksum: order-independent 64-bit sum over the texels of an output of a mix of (texel index, texel value), the formula
+//     hr_api.h states — lets a sharded run prove on the device that its gathered frame, or the sum of its ranks' own rows, equals the
+//     single-GPU frame.
 #include "hr_internal.h"
 
 namespace {
@@ -37,20 +38,24 @@ __device__ __forceinline__ unsigned long long mix64(unsigned long long z)
     return z ^ (z >> 31);
 }
 
-// words: the image as 32-bit words (every format here has rows that are multiples of 2 bytes; the byte count is passed and the
-// tail handled bytewise); word index is relative to the start of the IMAGE (not of the row range), so band sums add up.
-__global__ void k_checksum(const uint8_t* __restrict__ base, size_t byte0, size_t byte1, unsigned long long* __restrict__ out)
+// the texel's TS bytes as a little-endian unsigned integer (images are allocated with at least TS-byte alignment)
+template <int TS>
+__device__ __forceinline__ unsigned long long load_texel(const uint8_t* base, size_t i)
+{
+    if (TS == 1) return base[i];
+    if (TS == 2) return reinterpret_cast<const uint16_t*>(base)[i];
+    if (TS == 4) return reinterpret_cast<const uint32_t*>(base)[i];
+    return reinterpret_cast<const unsigned long long*>(base)[i];
+}
+
+// texels [t0, t1) of an image of TS-byte texels; texel i (row-major index from the start of the IMAGE, not of the row range) adds
+// mix64(mix64(i + 0x9E3779B97F4A7C15) ^ value), so the sums of any split of the rows add up to the whole image's (mod 2^64).
+template <int TS>
+__global__ void k_checksum(const uint8_t* __restrict__ base, size_t t0, size_t t1, unsigned long long* __restrict__ out)
 {
     unsigned long long acc = 0;
-    const size_t w0 = (byte0 + 3) / 4, w1 = byte1 / 4;
-    const uint32_t* w = reinterpret_cast<const uint32_t*>(base);
-    for (size_t i = w0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < w1; i += (size_t)gridDim.x * blockDim.x)
-        acc += mix64((i << 32) ^ (unsigned long long)w[i] ^ 0x9E3779B97F4A7C15ull);
-    if (blockIdx.x == 0 && threadIdx.x == 0)
-    { // unaligned head / tail bytes (byte ranges of whole rows of 1- or 2-byte texels)
-        for (size_t b = byte0; b < byte1 && b < w0 * 4; b++) acc += mix64(((b | (1ull << 40)) << 8) ^ base[b]);
-        for (size_t b = (w1 * 4 > byte0 ? w1 * 4 : byte0); b < byte1; b++) acc += mix64(((b | (1ull << 40)) << 8) ^ base[b]);
-    }
+    for (size_t i = t0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < t1; i += (size_t)gridDim.x * blockDim.x)
+        acc += mix64(mix64(i + 0x9E3779B97F4A7C15ull) ^ load_texel<TS>(base, i));
     // block reduction
     __shared__ unsigned long long s[32];
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xFFFFFFFFu, acc, o);
@@ -76,8 +81,15 @@ void launch_tile_stats(const uint8_t* flags, int TW, int t0, int t1, unsigned lo
 // out[0] = primary, out[1] = secondary rays since the last drain (counters reset)
 void launch_drain_ray_counters(unsigned long long* ctr, unsigned long long* d_out, cudaStream_t st) { k_drain_ray_counters<<<1, 64, 0, st>>>(ctr, d_out); }
 
-void launch_checksum(const void* base, size_t byte0, size_t byte1, unsigned long long* d_out, cudaStream_t st)
+void launch_checksum(const void* base, int texel_bytes, size_t texel0, size_t texel1, unsigned long long* d_out, cudaStream_t st)
 {
-    if (byte1 <= byte0) return;
-    k_checksum<<<296, 256, 0, st>>>(static_cast<const uint8_t*>(base), byte0, byte1, d_out);
+    if (texel1 <= texel0) return;
+    const uint8_t* b = static_cast<const uint8_t*>(base);
+    switch (texel_bytes)
+    {
+        case 1: k_checksum<1><<<296, 256, 0, st>>>(b, texel0, texel1, d_out); break;
+        case 2: k_checksum<2><<<296, 256, 0, st>>>(b, texel0, texel1, d_out); break;
+        case 4: k_checksum<4><<<296, 256, 0, st>>>(b, texel0, texel1, d_out); break;
+        default: k_checksum<8><<<296, 256, 0, st>>>(b, texel0, texel1, d_out); break;
+    }
 }

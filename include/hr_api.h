@@ -549,8 +549,10 @@ HR_API int hr_pass_upload(hr_pass* pass, int which, const void* host_src, size_t
 /* restart_accumulation() / clear_images() equivalent: next render behaves like first_frame for this pass's history. */
 HR_API int hr_pass_reset_history(hr_pass* pass);
 HR_API int hr_pass_destroy(hr_pass* pass);
-/* Per-stage GPU timings of the last render in ms (DW_SCOPED_SAMPLE equivalent, profiler.cpp:83-181).
- * Enable with hr_ctx_set_profiling(ctx,1); names/ms arrays of capacity cap; returns count via *n. Synchronises. */
+/* Per-stage GPU timings in ms (DW_SCOPED_SAMPLE equivalent, profiler.cpp:83-181) of the renders profiled since the previous call
+ * (at most the last 1024): one entry per stage name, in the order the names first occurred, each the mean over the renders that
+ * recorded that stage.  Enable with hr_ctx_set_profiling(ctx,1); names/ms arrays of capacity cap; returns count via *n.
+ * Synchronises. */
 HR_API int hr_ctx_set_profiling(hr_ctx* ctx, int enabled);
 HR_API int hr_pass_stage_times(hr_pass* pass, const char** names, float* ms, int cap, int* n);
 /* Test hook, process-wide.  key 1 = shadows a-trous implementation (0 naive global-memory kernel, 1 shared-memory tiled kernel,
@@ -568,8 +570,11 @@ HR_API uint64_t hr_ctx_launch_count(hr_ctx* ctx);
 
 /* Work actually done by a pass (bench.py: roofline on processed bytes, Mrays/s on counted rays; SURVEY.md §8d).
  * Ray counts accumulate on the device since the previous hr_pass_get_stats call (warp-aggregated atomics inside the trace
- * kernels); the tile counts describe the last render: 8x8 tiles of the rows this rank's denoise stages covered, and how many
- * of them were on the denoise list (the others take the reference's copy / zero-fill path).  Synchronises `stream`. */
+ * kernels), which drains them to 0; `renders` counts the same way.  The tile counts describe the last render only: the 8x8 tiles
+ * of the rows this rank's denoise stages covered (its band +- the denoise halo of hr_shard_halo_rows, the whole pass at world 1),
+ * and how many of them were on the denoise list (the others take the reference's copy / zero-fill path).  A render with
+ * denoise = 0 covers no rows: tiles_total, tiles_denoise and pixels_total are then 0.  Passes without tile flags (DDGI and the
+ * post passes) report 0 for them.  Synchronises `stream`. */
 typedef struct hr_pass_stats {
     uint64_t rays_primary;   /* K1/K7: pixels that traced a ray; K12: reflection rays; K18: probe rays                     */
     uint64_t rays_secondary; /* shadow / sky-light rays of the hit shading (K12, K18)                                      */
@@ -579,9 +584,15 @@ typedef struct hr_pass_stats {
     uint64_t renders;        /* renders since the previous call                                                           */
 } hr_pass_stats;
 HR_API int hr_pass_get_stats(hr_pass* pass, hr_pass_stats* out, void* stream);
-/* Order-independent 64-bit checksum of an output image computed on the device (sum over texels of a 64-bit mix of
- * (index, value)); rows [row0,row1) only, row1 <= 0 = whole image.  bench.py uses it to show that an N-GPU frame equals the
- * single-GPU frame without moving the images.  Synchronises `stream`. */
+/* Order-independent 64-bit checksum of an output image computed on the device, over rows [row0,row1) (row1 <= 0 = the whole
+ * image; any other range outside [0, height] or with row1 < row0 returns HR_ERR_INVALID_ARG):
+ *     sum mod 2^64 over the texels i of those rows of  mix(mix(i + 0x9E3779B97F4A7C15) ^ v_i)
+ * where i = y * width + x is the texel's row-major index from the image's first texel, v_i its 1, 2, 4 or 8 bytes (R8_UINT;
+ * R16F; R32_UINT, RG16F, RGBA8; RGBA16F) read as a little-endian unsigned integer, and mix the splitmix64 finaliser
+ *     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;  z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  mix(z) = z ^ (z >> 31).
+ * So the checksums of any split of the rows add up (mod 2^64) to the whole image's: the ranks of a sharded run can each sum their
+ * own rows.  bench.py uses it to show that an N-GPU frame equals the single-GPU frame without moving the images.  Synchronises
+ * `stream`. */
 HR_API int hr_pass_output_checksum(hr_pass* pass, int which, int row0, int row1, uint64_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

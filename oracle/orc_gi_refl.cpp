@@ -58,6 +58,7 @@ void ddgi_ray_trace(const ShadingScene& ss, const DDGIUniforms& d, const hr_fram
             vec3  L      = { 0, 0, 0 };
             float hit_distance = 10000.0f;
             Hit   h;
+            count_rays(0, 1);
             if (ss.scene->closest(origin, dir, 0.001f, 10000.0f, h))
             {
                 Surface s   = fetch_surface(ss, h);
@@ -252,6 +253,7 @@ void reflections_ray_trace(const ShadingScene& ss, const GBufLevel& g, const hr_
             if (trace)
             {
                 Hit h;
+                count_rays(0, 1);
                 if (ss.scene->closest(ray_origin, dir, 0.001f, 10000.0f, h))
                 {
                     Surface s  = fetch_surface(ss, h);

@@ -9,6 +9,7 @@
 #include "orc_constants.h"
 #include "orc_math.h"
 #include <algorithm>
+#include <atomic>
 #include <vector>
 
 namespace orc {
@@ -304,6 +305,12 @@ enum {
     ORC_RP_VIRTUAL  = 128  // reflections: virtual-point reprojection (else the motion vector); invalid = REACHED without ALL/SOME/FALLBACK
 };
 inline uint8_t*& reproject_codes() { static uint8_t* codes = nullptr; return codes; }
+
+// Rays the trace stages cast (tests only, orc_take_ray_counts): [0] primary, [1] secondary, the kinds of hr_pass_stats — K1 a ray
+// per sample whose light attenuation is > 0, K7 a ray per sample on geometry, K12 a reflection ray per traced sample (primary) and
+// direct_lighting's shadow / sky rays at its hits (secondary), K18 a ray per probe ray (primary) and its hits' direct_lighting rays.
+inline std::atomic<uint64_t>* ray_counts() { static std::atomic<uint64_t> c[2]; return c; }
+inline void count_rays(int kind, uint64_t n) { if (n) ray_counts()[kind].fetch_add(n, std::memory_order_relaxed); }
 
 template <int NC>
 inline bool reproject(const ReprojectIn& in, ReprojectOut& out)

@@ -32,7 +32,7 @@ void shadows_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f
     for (int my = 0; my < MH; my++)
         for (int mx = 0; mx < MW; mx++)
         {
-            uint32_t word = 0;
+            uint32_t word = 0, rays = 0;
             for (int li = 0; li < 32; li++)
             {
                 ivec2 c = { mx * 8 + (li & 7), my * 4 + (li >> 3) };
@@ -50,11 +50,12 @@ void shadows_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f
                     vec3  Wi;
                     float t_max, attenuation;
                     fetch_light_properties_shadow(f.ubo.light, world_pos, normal, rnd, Wi, t_max, attenuation);
-                    if (attenuation > 0.0f) result = (uint32_t)scene.query_visibility(ray_origin, Wi, t_max); // query_distance
+                    if (attenuation > 0.0f) { rays++; result = (uint32_t)scene.query_visibility(ray_origin, Wi, t_max); } // query_distance
                 }
                 word |= result << li;
             }
             mask[(size_t)my * MW + mx] = word;
+            count_rays(0, rays);
         }
 }
 
@@ -67,7 +68,7 @@ void ao_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f, flo
     for (int my = 0; my < MH; my++)
         for (int mx = 0; mx < MW; mx++)
         {
-            uint32_t word = 0;
+            uint32_t word = 0, rays = 0;
             for (int li = 0; li < 32; li++)
             {
                 ivec2 c = { mx * 8 + (li & 7), my * 4 + (li >> 3) };
@@ -77,6 +78,7 @@ void ao_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f, flo
                 uint32_t   result    = 0;
                 if (depth != 1.0f)
                 {
+                    rays++;
                     vec3 world_pos  = world_position_from_depth(tex_coord, depth, vpi);
                     vec4 gb2        = g.fetch2(c);
                     vec3 normal     = octohedral_to_direction({ gb2.x, gb2.y });
@@ -88,6 +90,7 @@ void ao_ray_trace(const Scene& scene, const GBufLevel& g, const hr_frame& f, flo
                 word |= result << li;
             }
             mask[(size_t)my * MW + mx] = word;
+            count_rays(0, rays);
         }
 }
 
@@ -106,7 +109,7 @@ void ray_trace_count(const Scene& scene, const GBufLevel& g, const hr_frame& f, 
             const ivec2 c = { x, y };
             const vec2  tex_coord = { ((float)c.x + 0.5f) / (float)g.W, ((float)c.y + 0.5f) / (float)g.H };
             const float depth = g.fetchd(c);
-            uint32_t    n = 0;
+            uint32_t    n = 0, rays = 0;
             if (depth != 1.0f)
             {
                 const vec3 world_pos  = world_position_from_depth(tex_coord, depth, vpi);
@@ -117,17 +120,18 @@ void ray_trace_count(const Scene& scene, const GBufLevel& g, const hr_frame& f, 
                 {
                     const uint32_t idx = f.num_frames * (uint32_t)spp + (uint32_t)s;
                     const vec2 rnd = { sample_blue_noise(c, idx, 0, bn), sample_blue_noise(c, idx, 1, bn) };
-                    if (ao) n += (uint32_t)scene.query_visibility(ray_origin, sample_cosine_lobe(normal, rnd), p0);
+                    if (ao) { rays++; n += (uint32_t)scene.query_visibility(ray_origin, sample_cosine_lobe(normal, rnd), p0); }
                     else
                     {
                         vec3  Wi;
                         float t_max, attenuation;
                         fetch_light_properties_shadow(f.ubo.light, world_pos, normal, rnd, Wi, t_max, attenuation);
-                        if (attenuation > 0.0f) n += (uint32_t)scene.query_visibility(ray_origin, Wi, t_max);
+                        if (attenuation > 0.0f) { rays++; n += (uint32_t)scene.query_visibility(ray_origin, Wi, t_max); }
                     }
                 }
             }
             count[(size_t)y * g.W + x] = (uint8_t)n;
+            count_rays(0, rays);
         }
 }
 
@@ -475,6 +479,12 @@ extern "C" {
 
 // record reproject()'s branches (ORC_RP_* bits, orc_glsl.h) into `codes` (one byte per pixel of the next temporal stage's pass), or stop (NULL)
 void orc_set_reproject_codes(uint8_t* codes) { reproject_codes() = codes; }
+
+// the rays counted since the previous call (ray_counts, orc_glsl.h): out[0] primary, out[1] secondary; the counts restart at 0
+void orc_take_ray_counts(uint64_t* out)
+{
+    for (int k = 0; k < 2; k++) out[k] = ray_counts()[k].exchange(0);
+}
 
 struct orc_gbuf { int32_t W, H; const uint16_t* gb2; const uint16_t* gb3; const float* depth; };
 static GBufLevel lvl(const orc_gbuf* g) { GBufLevel l; l.W = g->W; l.H = g->H; l.gb2 = g->gb2; l.gb3 = g->gb3; l.depth = g->depth; return l; }

@@ -220,7 +220,7 @@ inline vec3 direct_lighting(const Scene& scene, const hr_light& light, vec3 Wo, 
         float t_max, attenuation;
         fetch_light_properties_hard(light, P, N, Li, Wi, t_max, attenuation);
         vec3 Wh = normalize(Wo + Wi);
-        if (attenuation > 0.0f) attenuation *= scene.query_visibility(ray_origin, Wi, t_max); // query_distance :172
+        if (attenuation > 0.0f) { count_rays(1, 1); attenuation *= scene.query_visibility(ray_origin, Wi, t_max); } // query_distance :172
         vec3 brdf = evaluate_uber_brdf(diffuse_color, roughness, N, F0, Wo, Wh, Wi);
         Lo = Lo + (brdf * attenuation) * Li;
     }
@@ -229,6 +229,7 @@ inline vec3 direct_lighting(const Scene& scene, const hr_light& light, vec3 Wo, 
         vec3 Wi = sample_cosine_lobe(N, rng2);
         vec3 Li = sky_color; // texture(sky_cubemap, Wi): constant-colour environment
         vec3 Wh = normalize(Wo + Wi);
+        count_rays(1, 1);
         Li      = Li * scene.query_visibility(ray_origin, Wi, 10000.0f);
         vec3 brdf = evaluate_uber_brdf(diffuse_color, roughness, N, F0, Wo, Wh, Wi);
         Lo = Lo + brdf * Li;

@@ -83,6 +83,7 @@ def lib():
         L.orc_texture_sample.argtypes = [P, P, C.c_size_t, P]
         L.orc_fetch_material.argtypes = [P, P, P, C.c_size_t, P]
         L.orc_set_reproject_codes.argtypes = [P]
+        L.orc_take_ray_counts.argtypes = [P]
         _lib = L
     return _lib
 
@@ -345,6 +346,14 @@ class ReprojectCodes:
         out["invalid"] = int(np.count_nonzero((c & 1) & ((c & (8 | 16 | 64)) == 0)))
         out["motion"] = out["reached"] - out["virtual"]
         return out
+
+
+def take_ray_counts():
+    """(primary, secondary) rays the oracle's trace stages cast since the previous call, counted as the device's hr_pass_stats
+    counts them (oracle/orc_glsl.h ray_counts); the counts restart at 0"""
+    out = np.zeros(2, np.uint64)
+    lib().orc_take_ray_counts(p(out))
+    return int(out[0]), int(out[1])
 
 
 def h2f(a):
