@@ -870,8 +870,7 @@ static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const 
     int          rc;
     if (shared)
     {
-        if (spp > 1) launch_ray_trace_count_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), count, spp, rts, fr.st);
-        else launch_ray_trace_mask_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, rts, fr.st);
+        launch_ray_trace_shared(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), count, spp, rts, fr.st);
         ctx->launches++;
         if ((rc = hr_rt_share_finish(p, parity, fr.epoch, spp > 1, fr.st)) != HR_OK) return rc;
         timer_mark(p, "Ray Trace", fr.st);
@@ -882,13 +881,10 @@ static int trace_mask(hr_pass* p, PassFrame& fr, const GBufLevelDev& cur, const 
     }
     else
     {
-        if (spp > 1)
-        { // SURVEY.md §8d: spp rays per pixel into an 8-bit count image (allocated on first use)
-            if (!p->count && (rc = pass_alloc(p, p->count, (size_t)p->W * p->H)) != HR_OK) return rc;
-            count = p->count;
-            launch_ray_trace_count(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), count, spp, fr.rt0, fr.rt1, fr.st);
-        }
-        else launch_ray_trace_mask(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, ctx->d_scr_rank, mask, fr.rt0, fr.rt1, fr.st);
+        // SURVEY.md §8d: with spp > 1, spp rays per pixel into an 8-bit count image (allocated on first use)
+        if (spp > 1 && !p->count && (rc = pass_alloc(p, p->count, (size_t)p->W * p->H)) != HR_OK) return rc;
+        count = p->count;
+        launch_ray_trace(p->kind, cur, bvh, fc, p0, p1, ctx->d_sobol, bn_table(ctx, spp), mask, count, spp, fr.rt0, fr.rt1, fr.st);
         ctx->launches++;
         timer_mark(p, "Ray Trace", fr.st);
         // the history = last frame's images of whichever rank owns the reprojected row (peer history, shard.cu): wait until every
@@ -1001,10 +997,8 @@ int hr_shadows_render(hr_pass* p, const hr_frame* f, const hr_shadows_params* pr
         // History = prev_image[!pp] / moments[!pp] of whichever rank owns the reprojected row (peer history, shard.cu).
         HistPeers hist;
         hr_peer_hist(p, SHARED_HIST + !pp, SHARED_HIST_AUX + !pp, p->H, fr.no_history, &hist);
-        if (spp > 1)
-            launch_shadows_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
-        else
-            launch_shadows_temporal(cur, prev, mask, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags, fr.row0, fr.row1, st);
+        launch_temporal(PASS_SHADOWS, cur, prev, mask, count, spp, hist, fc, prm->alpha, prm->moments_alpha, p->temporal_out, p->moments[pp], p->tile_flags,
+                        fr.row0, fr.row1, st);
         ctx->launches++;
         timer_mark(p, "Temporal Accumulation", st);
         // a_trous_filter (:1094-1215).  The reference ping-pongs image[0]/image[1] and copies the output of
@@ -1133,8 +1127,7 @@ int hr_ao_render(hr_pass* p, const hr_frame* f, const hr_ao_params* prm, void* s
         // history = ao_color[!pp] / ao_len[!pp] of the rank that owns the reprojected row (peer history, shard.cu)
         HistPeers hist;
         hr_peer_hist(p, SHARED_HIST + !pp, SHARED_HIST_AUX + !pp, p->H, fr.no_history, &hist);
-        if (spp > 1) launch_ao_temporal_count(cur, prev, count, spp, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
-        else launch_ao_temporal(cur, prev, mask, hist, fc, prm->alpha, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
+        launch_temporal(PASS_AO, cur, prev, mask, count, spp, hist, fc, prm->alpha, 0.0f, p->ao_color[pp], p->ao_len[pp], p->tile_flags, fr.row0, fr.row1, st);
         ctx->launches++;
         if ((rc = frame_signal(p, fr)) != HR_OK) return rc; // this frame's history (ao_color[pp], ao_len[pp]) is complete
         timer_mark(p, "Temporal Accumulation", st);

@@ -391,31 +391,22 @@ inline bool hr_once_per_device(bool (&done)[64])
 }
 
 
-void launch_shadows_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
-                                   float alpha, float moments_alpha, __half2* out, uint2* moments_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
-void launch_ao_temporal_count(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint8_t* count, int spp, const HistPeers& hist, const FrameConsts& fc,
-                              float alpha, __half* out, __half* len_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
-// trace.cu: the shadows (kind PASS_SHADOWS, K1: p0 = bias) and AO (PASS_AO, K7: p0 = ray length, p1 = bias) ray traces into the mask image,
-// the mask images of the cooperative trace (shard.cu) or, spp > 1, the count image (band-local or cooperative)
-void launch_ray_trace_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
-                           uint32_t* mask, int row0, int row1, cudaStream_t st);
-void launch_ray_trace_mask_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
-                                  const uint8_t* sr, const RtShare& sh, cudaStream_t st);
-void launch_ray_trace_count_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
-                                   const uint8_t* sr, uint8_t* count, int spp, const RtShare& sh, cudaStream_t st);
-void launch_ray_trace_count(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
-                            uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
+// trace.cu: the shadows (kind PASS_SHADOWS, K1: p0 = bias) and AO (PASS_AO, K7: p0 = ray length, p1 = bias) ray traces into the mask image
+// or, spp > 1, the count image: band-local, or this rank's share of the cooperative trace (shard.cu; mask words to sh.mask_local)
+void launch_ray_trace(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol, const uint8_t* sr,
+                      uint32_t* mask, uint8_t* count, int spp, int row0, int row1, cudaStream_t st);
+void launch_ray_trace_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, const uint8_t* sobol,
+                             const uint8_t* sr, uint8_t* count, int spp, const RtShare& sh, cudaStream_t st);
 void launch_trace_any(const BvhDev& bvh, const float* rays, size_t n, uint32_t* out, cudaStream_t st);
 void launch_trace_closest(const BvhDev& bvh, const float* rays, size_t n, float* out_t, uint32_t* out_prim, float* out_uv, cudaStream_t st);
 
-void launch_shadows_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint32_t* mask, const HistPeers& hist,
-                             const FrameConsts& fc, float alpha, float moments_alpha, __half2* out, uint2* moments_out, uint8_t* tile_flags,
-                             int row0, int row1, cudaStream_t st);
+// svgf_temporal.cu: K3 (PASS_SHADOWS: out_img RG16F, out_aux moments RGBA16F) or K9 (PASS_AO: out_img R16F, out_aux history length
+// R16F; moments_alpha unused), the visibility from `mask` at spp 1 or from `count` at spp > 1
+void launch_temporal(int kind, const GBufLevelDev& cur, const GBufLevelDev& prev, const uint32_t* mask, const uint8_t* count, int spp, const HistPeers& hist,
+                     const FrameConsts& fc, float alpha, float moments_alpha, void* out_img, void* out_aux, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st);
 void launch_upsample_scalar(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, int in_channels, float sky_value, float power,
                             __half* out, int row0, int row1, cudaStream_t st);
-void launch_ao_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const uint32_t* mask, const HistPeers& hist,
-                        const FrameConsts& fc, float alpha, __half* out, __half* len_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 void launch_ao_blur(const GBufLevelDev& g, const __half* in, const uint8_t* tile_flags, const float* zbp, int dirx, int diry, int radius, __half* out,
                     int row0, int row1, cudaStream_t st);

@@ -6,6 +6,7 @@ N ranks are emulated on one GPU (one hr_ctx per rank, hr_shard_config + hr_shard
 wait for each other inside a frame); test_nccl_* is the one-process-per-GPU run and needs >= 2 GPUs.
 """
 import os
+import re
 
 import numpy as np
 import pytest
@@ -266,8 +267,9 @@ def test_cost_balancing_above_1024_mask_rows():
 
 
 @pytest.mark.parametrize("kind", ["shadows", "ao", "reflections"])
-def test_launch_count_linked_spp2(kind):
-    """hr_ctx_launch_count over a linked spp = 2 pair equals the kernels torch.profiler records"""
+def test_launch_count_linked_spp2_trace_kernel(kind):
+    """hr_ctx_launch_count over a linked spp = 2 pair equals the kernels torch.profiler records, and the ray trace among them is
+    the cooperative multi-sample one"""
     sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
     ctxs = [_ctx(sc, r, 2) for r in range(2)]
     if kind == "reflections":
@@ -301,7 +303,9 @@ def test_launch_count_linked_spp2(kind):
         one()  # first frame: history clears, peer mapping
         names = kernels_launched(one)
         assert len(names) == state["launches"], f"{kind}: {state['launches']} launches counted, {len(names)} kernels recorded: {names}"
-        assert any(("count_shared" if kind != "reflections" else "reflections_ray_trace") in n for n in names), names
+        # shadows / AO: the cooperative trace in its count form, k_ray_trace_shared<MODE, true> however the name is (de)mangled
+        coop = r"k_ray_trace_shared(<[^,>]*, ?(true|\(bool\)1)>|ILi\dELb1E)" if kind != "reflections" else "reflections_ray_trace"
+        assert any(re.search(coop, n) for n in names), names
     finally:
         _close(ctxs, ps)
 

@@ -1,7 +1,7 @@
 """spp > 1 (SURVEY.md §8d configs 4-5; NOT in the reference): `spp` rays per pixel with sample index num_frames * spp + s, an
 8-bit image of unoccluded-ray counts instead of the 1-bit mask, visibility = count / spp in the temporal stage.
 
-The CUDA kernels of this mode (k_ray_trace_count, k_temporal_count) mirror the validated 1-spp kernels; the ray counts must be
+This mode runs the COUNT forms of the 1-spp kernels (k_ray_trace<MODE, true>, k_temporal<MODE, PEER, true>); the ray counts must be
 exact against the oracle and the denoised images within the same tolerances as the 1-spp chains.
 """
 import numpy as np

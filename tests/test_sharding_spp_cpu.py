@@ -1,5 +1,5 @@
 """CPU, gloo world 2 / 3: the cooperative multi-sample (spp > 1) ray trace restated on the oracle (DESIGN.md §9).  Each rank traces an
-arbitrary, frame-varying share of the count image's mask rows (4 image rows each) — what k_ray_trace_count_shared does with the
+arbitrary, frame-varying share of the count image's mask rows (4 image rows each) — what k_ray_trace_shared<MODE, true> does with the
 cost-balanced partition — and the shares are exchanged so that every rank holds the complete count image (k_rt_push).  The
 denoise stages then run on band +- halo with the history of each rank valid on its own band only; the result must equal the
 whole-image oracle bit for bit.
