@@ -303,6 +303,9 @@ void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& pr
                                  float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 int  launch_reflections_atrous(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
                                float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st);
+// svgf_refl_atrous_v2.cu: the pixel-pair kernels of launch_reflections_atrous; false when they do not support the call
+bool launch_reflections_atrous_v2(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
+                                  float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st);
 void launch_upsample_vec4(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, void* out, int row0, int row1, cudaStream_t st);
 
 // ---- row-band sharding (shard.cu) ---------------------------------------------------------------------
@@ -406,6 +409,9 @@ void launch_temporal(int kind, const GBufLevelDev& cur, const GBufLevelDev& prev
                      const FrameConsts& fc, float alpha, float moments_alpha, void* out_img, void* out_aux, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st);
+// svgf_atrous_v3.cu: the pixel-pair kernels of launch_shadows_atrous; false when they do not support the call
+bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n, float sigma_z,
+                              float power, uint32_t* out, int row0, int row1, cudaStream_t st);
 void launch_upsample_scalar(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, int in_channels, float sky_value, float power,
                             __half* out, int row0, int row1, cudaStream_t st);
 void launch_ao_blur(const GBufLevelDev& g, const __half* in, const uint8_t* tile_flags, const float* zbp, int dirx, int diry, int radius, __half* out,

@@ -191,8 +191,6 @@ void launch_tiled(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, 
 // 3 = pixel-pair kernel (svgf_atrous_v3.cu, default); it falls back to the
 // scalar tiled kernel for odd widths / phi_normal != 32.
 int g_hr_atrous_impl = 3;
-bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n, float sigma_z,
-                              float power, uint32_t* out, int row0, int row1, cudaStream_t st); // svgf_atrous_v3.cu (impl 3: pixel pairs)
 
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st)

@@ -1,24 +1,17 @@
-// svgf_refl_atrous_v2.cu — reflections a-trous (K15 + K16, reflections_denoise_atrous.comp:94-181) on pixel pairs.
+// svgf_refl_atrous_v2.cu — reflections a-trous (K15 + K16, reflections_denoise_atrous.comp:94-181) on pixel pairs
+// (atrous_pairs.cuh).
 //
-// This is the roofline kernel of BASELINE config 3 (4K full-res reflections: 36 algorithmic B/px/iteration, SURVEY.md §8d).  The
-// scalar kernel (svgf_reflections.cu::k_refl_atrous) is instruction-issue bound like its shadows twin was; this one applies the
-// same remedy as svgf_atrous_v3.cu: every thread filters TWO horizontally adjacent pixels and keeps each per-pixel quantity of
-// the pair in one 64-bit register pair (gf::ffma2 / fmul2 / fadd2), so addressing, shared-memory loads and loop overhead are
-// shared by both pixels.  Shared memory holds the staged tile + halo as nine fp32 planes (nx, ny, nz, z * log2e / sigma, r, g, b,
-// variance, luminance — the sample luminance is computed once per staged texel instead of once per tap); an aligned LDS.64
-// fetches a plane value for both pixels of a pair.  Out-of-image cells are staged with a zero normal (weight 0 = the
-// reference's `inside` test) and zero colour / variance (texelFetch robust-access zeros for compute_variance_center).
+// This is the roofline kernel of BASELINE config 3 (4K full-res reflections: 36 algorithmic B/px/iteration, SURVEY.md §8d).
+// Nine staged planes: nx, ny, nz, z * log2e / sigma, r, g, b, variance, luminance (the sample luminance is computed once per
+// staged texel instead of once per tap).
 // Tile classification (K13/K15): tiles whose flag is 0 are copied (reflections_denoise_copy_tiles.comp:35-38).
-#include "glsl_fast.cuh"
-#include "hr_internal.h"
+#include "atrous_pairs.cuh"
 #include <cuda.h> // CUtensorMap (driver types only; cuTensorMapEncodeTiled is fetched with cudaGetDriverEntryPoint)
 #include <vector>
 
 namespace {
 
 using namespace gf;
-
-constexpr int TWR = 64, THR = 16, NPL = 9;
 
 struct R2Params {
     int   W, H;
@@ -28,124 +21,7 @@ struct R2Params {
     int   row0, row1;
 };
 
-__device__ __forceinline__ float2 ldp(const float* __restrict__ plane, int idx, bool aligned)
-{
-    if (aligned) return *reinterpret_cast<const float2*>(plane + idx);
-    return make_float2(plane[idx], plane[idx + 1]);
-}
-
 __device__ __forceinline__ float lum3(float r, float g, float b) { return fmaxf(r * 0.299f + g * 0.587f + b * 0.114f, 0.0001f); } // common.glsl:143
-
-// Stage the texel pair (px, px+1) of row py (px even) at region index ri (even).
-__device__ __forceinline__ void stage_pair9(const GBufLevelDev& g, const uint2* __restrict__ in, float c_sigma, int px, int py, int W, int H, int ri, float* s, int PL)
-{
-    float2 nx = make_float2(0.0f, 0.0f), ny = nx, nz = nx, zs = nx, cr = nx, cg = nx, cb = nx, va = nx, lu = make_float2(0.0001f, 0.0001f);
-    if (px >= 0 && py >= 0 && px < W && py < H)
-    {
-        const size_t pi = (size_t)py * W + px;
-        const uint4  a  = __ldg(reinterpret_cast<const uint4*>(g.gb2 + pi)); // two RGBA16F texels: .x / .z hold the oct normals
-        const uint4  b  = __ldg(reinterpret_cast<const uint4*>(g.gb3 + pi)); // .y / .w hold (mesh id, linear z)
-        const uint4  c  = __ldg(reinterpret_cast<const uint4*>(in + pi));    // two RGBA16F texels (rgb, variance)
-        const float2 e0 = h2_to_f2(a.x), e1 = h2_to_f2(a.z);
-        const float3 n0 = octohedral_to_direction(e0.x, e0.y), n1 = octohedral_to_direction(e1.x, e1.y);
-        const float2 c0 = h2_to_f2(c.x), c1 = h2_to_f2(c.y), c2 = h2_to_f2(c.z), c3 = h2_to_f2(c.w);
-        nx = make_float2(n0.x, n1.x); ny = make_float2(n0.y, n1.y); nz = make_float2(n0.z, n1.z);
-        zs = make_float2(h2_to_f2(b.y).y * c_sigma, h2_to_f2(b.w).y * c_sigma);
-        cr = make_float2(c0.x, c2.x); cg = make_float2(c0.y, c2.y); cb = make_float2(c1.x, c3.x); va = make_float2(c1.y, c3.y);
-        lu = make_float2(lum3(c0.x, c0.y, c1.x), lum3(c2.x, c2.y, c3.x));
-    }
-    float* p = s + ri;
-    *reinterpret_cast<float2*>(p) = nx; p += PL;
-    *reinterpret_cast<float2*>(p) = ny; p += PL;
-    *reinterpret_cast<float2*>(p) = nz; p += PL;
-    *reinterpret_cast<float2*>(p) = zs; p += PL;
-    *reinterpret_cast<float2*>(p) = cr; p += PL;
-    *reinterpret_cast<float2*>(p) = cg; p += PL;
-    *reinterpret_cast<float2*>(p) = cb; p += PL;
-    *reinterpret_cast<float2*>(p) = va; p += PL;
-    *reinterpret_cast<float2*>(p) = lu;
-}
-
-// Filter one pixel pair whose centre cell is at region index ci; row / column tap strides in cells are (rs, cs).
-// vrow_up / vrow_dn: region indices of the cells directly above / below the centre at UNIT pixel spacing in the variance plane
-// given by vplane_up / vplane_dn (the dense tile keeps them in the main variance plane; the row-interleaved tile in side buffers).
-template <bool ALIGNED_X>
-__device__ __forceinline__ void filter_pair(const float* __restrict__ s, int PL, int ci, int rs, int cs, const float* __restrict__ v_up, const float* __restrict__ v_dn,
-                                            float c_phi0, float2& o_r, float2& o_g, float2& o_b, float2& o_v, float2& c_zs)
-{
-    const float* s_nx = s;
-    const float* s_ny = s + PL;
-    const float* s_nz = s + 2 * PL;
-    const float* s_zs = s + 3 * PL;
-    const float* s_r  = s + 4 * PL;
-    const float* s_g  = s + 5 * PL;
-    const float* s_b  = s + 6 * PL;
-    const float* s_va = s + 7 * PL;
-    const float* s_lu = s + 8 * PL;
-    const float2 cnx = ldp(s_nx, ci, true), cny = ldp(s_ny, ci, true), cnz = ldp(s_nz, ci, true), czs = ldp(s_zs, ci, true);
-    const float2 ccr = ldp(s_r, ci, true), ccg = ldp(s_g, ci, true), ccb = ldp(s_b, ci, true), cva = ldp(s_va, ci, true), clu = ldp(s_lu, ci, true);
-    c_zs = czs;
-    // compute_variance_center for both pixels (:65-88): columns ci-1 .. ci+2, rows -1..+1 at unit spacing; weights {1/4,1/8,1/16}
-    float2 vbar;
-    {
-        const float  a0 = v_up[-1], d0 = v_up[2];
-        const float2 m0 = *reinterpret_cast<const float2*>(v_up);
-        const float  a1 = s_va[ci - 1], d1 = s_va[ci + 2];
-        const float  a2 = v_dn[-1], d2 = v_dn[2];
-        const float2 m2 = *reinterpret_cast<const float2*>(v_dn);
-        vbar.x = 0.25f * cva.x + 0.125f * (a1 + cva.y + m0.x + m2.x) + 0.0625f * (a0 + m0.y + a2 + m2.y);
-        vbar.y = 0.25f * cva.y + 0.125f * (cva.x + d1 + m0.y + m2.y) + 0.0625f * (m0.x + d0 + m2.x + d2);
-    }
-    const float2 cphi = make_float2(c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.x, 1e-30f)), c_phi0 * rsqrtf(fmaxf(1e-10f + vbar.y, 1e-30f)));
-    const float2 neg1 = make_float2(-1.0f, -1.0f), nl2e = make_float2(-1.44269504f, -1.44269504f);
-    const float  LK1 = -0.5849625007f, LK2 = -1.1699250014f; // log2(2/3), log2(4/9): kernel weights folded into the exponent
-    float2 sumw = make_float2(1.0f, 1.0f), ar = ccr, ag = ccg, ab = ccb, av = cva;
-#pragma unroll
-    for (int yy = -1; yy <= 1; yy++)
-#pragma unroll
-        for (int xx = -1; xx <= 1; xx++)
-        {
-            if (xx == 0 && yy == 0) continue;
-            const float lk = (xx != 0 && yy != 0) ? LK2 : LK1;
-            const int   si = ci + yy * rs + xx * cs;
-            const bool  al = ALIGNED_X || xx == 0;
-            const float2 snx = ldp(s_nx, si, al), sny = ldp(s_ny, si, al), snz = ldp(s_nz, si, al), szs = ldp(s_zs, si, al);
-            const float2 sr = ldp(s_r, si, al), sg = ldp(s_g, si, al), sb = ldp(s_b, si, al), sv = ldp(s_va, si, al), sl = ldp(s_lu, si, al);
-            const float2 dz = ffma2(szs, neg1, czs);
-            float2       wZ;
-            wZ.x = fast_exp2(-fabsf(dz.x));
-            wZ.y = fast_exp2(-fabsf(dz.y));
-            const float2 dl = ffma2(sl, neg1, clu);
-            float2       ea;
-            ea.x = fmaf(fabsf(dl.x), cphi.x, lk);
-            ea.y = fmaf(fabsf(dl.y), cphi.y, lk);
-            ea   = ffma2(wZ, nl2e, ea);
-            float2 e;
-            e.x = fast_exp2(ea.x);
-            e.y = fast_exp2(ea.y);
-            float2 nd = fmul2(cnz, snz);
-            nd        = ffma2(cny, sny, nd);
-            nd        = ffma2(cnx, snx, nd);
-            nd.x      = fmaxf(nd.x, 0.0f);
-            nd.y      = fmaxf(nd.y, 0.0f);
-            float2 p = fmul2(nd, nd);
-            p        = fmul2(p, p);
-            p        = fmul2(p, p);
-            p        = fmul2(p, p);
-            p        = fmul2(p, p);
-            const float2 wk = fmul2(e, p);
-            sumw = fadd2(sumw, wk);
-            ar   = ffma2(wk, sr, ar);
-            ag   = ffma2(wk, sg, ag);
-            ab   = ffma2(wk, sb, ab);
-            av   = ffma2(fmul2(wk, wk), sv, av);
-        }
-    const float2 inv = make_float2(fast_rcp(sumw.x), fast_rcp(sumw.y));
-    o_r = fmul2(ar, inv);
-    o_g = fmul2(ag, inv);
-    o_b = fmul2(ab, inv);
-    o_v = fmul2(fmul2(av, inv), inv);
-}
 
 // per-pixel class of the reference's early-outs (:119-128): 0 = sky -> 0, 1 = mirror / DDGI-rough -> pass-through, 2 = filter
 __device__ __forceinline__ int pixel_class(float depth, float roughness, int approx)
@@ -155,205 +31,97 @@ __device__ __forceinline__ int pixel_class(float depth, float roughness, int app
     return 2;
 }
 
-__device__ __forceinline__ void store_pair(uint2* __restrict__ out, size_t idx, bool has1, int k0, int k1, const float* __restrict__ s, int PL, int ci, float2 o_r, float2 o_g,
-                                           float2 o_b, float2 o_v)
+__device__ __forceinline__ void store_pair(uint2* __restrict__ out, size_t idx, bool has1, int k0, int k1, const float* __restrict__ s, int PL, int ci, const PairSum<3>& f)
 {
-    const float2 ccr = ldp(s + 4 * PL, ci, true), ccg = ldp(s + 5 * PL, ci, true), ccb = ldp(s + 6 * PL, ci, true), cva = ldp(s + 7 * PL, ci, true);
+    const float2 ccr = ld_pair(s + 4 * PL, ci, true), ccg = ld_pair(s + 5 * PL, ci, true), ccb = ld_pair(s + 6 * PL, ci, true), cva = ld_pair(s + 7 * PL, ci, true);
     uint2 r0, r1;
     if (k0 == 0) r0 = make_uint2(0u, 0u);
     else if (k0 == 1) r0 = make_uint2(f2_to_h2(ccr.x, ccg.x), f2_to_h2(ccb.x, cva.x));
-    else r0 = make_uint2(f2_to_h2(o_r.x, o_g.x), f2_to_h2(o_b.x, o_v.x));
+    else r0 = make_uint2(f2_to_h2(f.c[0].x, f.c[1].x), f2_to_h2(f.c[2].x, f.v.x));
     if (k1 == 0) r1 = make_uint2(0u, 0u);
     else if (k1 == 1) r1 = make_uint2(f2_to_h2(ccr.y, ccg.y), f2_to_h2(ccb.y, cva.y));
-    else r1 = make_uint2(f2_to_h2(o_r.y, o_g.y), f2_to_h2(o_b.y, o_v.y));
+    else r1 = make_uint2(f2_to_h2(f.c[0].y, f.c[1].y), f2_to_h2(f.c[2].y, f.v.y));
     if (has1) *reinterpret_cast<uint4*>(out + idx) = make_uint4(r0.x, r0.y, r1.x, r1.y); // idx even (W even is required by the launcher)
     else out[idx] = r0;
 }
 
-// Dense tile: 64x16 pixels + STEP halo.  Registers are tuned for 4 resident CTAs per SM: they hide the staging latency.
+struct ReflectionsPass {
+    using In = uint2; using Out = uint2; using Params = R2Params;
+    static constexpr int  NPL = 9, NC = 3;
+    static constexpr bool COPY_EMPTY_CTA = true; // a CTA whose tiles are all unflagged copies in -> out
+
+    // Stage the texel pair (px, px+1) of row py (px even) at region index ri (even).
+    static __device__ __forceinline__ void stage(const GBufLevelDev& g, const uint2* __restrict__ in, float c_sigma, int px, int py, int W, int H, int ri, float* s, int PL)
+    {
+        float2 nx = make_float2(0.0f, 0.0f), ny = nx, nz = nx, zs = nx, cr = nx, cg = nx, cb = nx, va = nx, lu = make_float2(0.0001f, 0.0001f);
+        if (px >= 0 && py >= 0 && px < W && py < H)
+        {
+            const size_t pi = (size_t)py * W + px;
+            const uint4  a  = __ldg(reinterpret_cast<const uint4*>(g.gb2 + pi)); // two RGBA16F texels: .x / .z hold the oct normals
+            const uint4  b  = __ldg(reinterpret_cast<const uint4*>(g.gb3 + pi)); // .y / .w hold (mesh id, linear z)
+            const uint4  c  = __ldg(reinterpret_cast<const uint4*>(in + pi));    // two RGBA16F texels (rgb, variance)
+            const float2 e0 = h2_to_f2(a.x), e1 = h2_to_f2(a.z);
+            const float3 n0 = octohedral_to_direction(e0.x, e0.y), n1 = octohedral_to_direction(e1.x, e1.y);
+            const float2 c0 = h2_to_f2(c.x), c1 = h2_to_f2(c.y), c2 = h2_to_f2(c.z), c3 = h2_to_f2(c.w);
+            nx = make_float2(n0.x, n1.x); ny = make_float2(n0.y, n1.y); nz = make_float2(n0.z, n1.z);
+            zs = make_float2(h2_to_f2(b.y).y * c_sigma, h2_to_f2(b.w).y * c_sigma);
+            cr = make_float2(c0.x, c2.x); cg = make_float2(c0.y, c2.y); cb = make_float2(c1.x, c3.x); va = make_float2(c1.y, c3.y);
+            lu = make_float2(lum3(c0.x, c0.y, c1.x), lum3(c2.x, c2.y, c3.x));
+        }
+        float* p = s + ri;
+        *reinterpret_cast<float2*>(p) = nx; p += PL;
+        *reinterpret_cast<float2*>(p) = ny; p += PL;
+        *reinterpret_cast<float2*>(p) = nz; p += PL;
+        *reinterpret_cast<float2*>(p) = zs; p += PL;
+        *reinterpret_cast<float2*>(p) = cr; p += PL;
+        *reinterpret_cast<float2*>(p) = cg; p += PL;
+        *reinterpret_cast<float2*>(p) = cb; p += PL;
+        *reinterpret_cast<float2*>(p) = va; p += PL;
+        *reinterpret_cast<float2*>(p) = lu;
+    }
+
+    static __device__ __forceinline__ float2 side_var(const uint2* __restrict__ in, size_t pi)
+    {
+        const uint4 w = __ldg(reinterpret_cast<const uint4*>(in + pi));
+        return make_float2(h2_to_f2(w.y).y, h2_to_f2(w.w).y);
+    }
+
+    static __device__ __forceinline__ void copy(const uint2* __restrict__ in, uint2* __restrict__ out, size_t idx, bool has1)
+    {
+        if (has1) *reinterpret_cast<uint4*>(out + idx) = __ldg(reinterpret_cast<const uint4*>(in + idx));
+        else out[idx] = __ldg(in + idx);
+    }
+
+    template <bool ALIGNED_X>
+    static __device__ __forceinline__ void filter_store(const GBufLevelDev& g, const R2Params& P, const PairTaps& t, uint2* __restrict__ out, size_t idx, bool has1, bool flagged)
+    {
+        int k0 = 1, k1 = 1; // copy tile: pass-through
+        if (flagged)
+        {
+            const float2 d  = has1 ? __ldg(reinterpret_cast<const float2*>(g.depth + idx)) : make_float2(__ldg(g.depth + idx), 1.0f);
+            const float  r0 = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx))).x;
+            const float  r1 = has1 ? h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx + 1))).x : 0.0f;
+            k0 = pixel_class(d.x, r0, P.approx);
+            k1 = has1 ? pixel_class(d.y, r1, P.approx) : 0;
+        }
+        PairSum<3> f = {};
+        if (k0 == 2 || k1 == 2) f = filter_pair<3, 8, ALIGNED_X>(t, P.c_phi0); // plane 8: luminance
+        store_pair(out, idx, has1, k0, k1, t.s, t.PL, t.ci, f);
+    }
+};
+
+// Dense tile.  Registers are tuned for 4 resident CTAs per SM: they hide the staging latency.
 template <int STEP>
 __global__ void __launch_bounds__(256, 4) k_refl_atrous_v2(GBufLevelDev g, const uint2* __restrict__ in, const uint8_t* __restrict__ tile_flags, R2Params P, uint2* __restrict__ out)
 {
-    extern __shared__ float smem_f[];
-    constexpr int PADL = STEP + (STEP & 1);            // even left pad => even region column for even image column
-    constexpr int RW   = (TWR + PADL + STEP + 1) & ~1; // even row pitch keeps LDS.64 alignment on every row
-    constexpr int RH   = THR + 2 * STEP;
-    constexpr int PL   = RW * RH;
-    __shared__ uint32_t s_tf;
-    const int W = P.W, H = P.H;
-    const int x0 = blockIdx.x * TWR, y0 = P.row0 + blockIdx.y * THR;
-    const int TWt = (W + 7) >> 3, THt = (H + 7) >> 3;
-    if (threadIdx.x < 32)
-    {
-        const int  tx = (x0 >> 3) + (threadIdx.x & 7), ty = (y0 >> 3) + (threadIdx.x >> 3);
-        const bool f  = threadIdx.x < 16 && tx < TWt && ty < THt && tile_flags[(size_t)ty * TWt + tx] != 0;
-        const uint32_t b = __ballot_sync(0xFFFFFFFFu, f);
-        if (threadIdx.x == 0) s_tf = b;
-    }
-    __syncthreads();
-    const uint32_t tf = s_tf;
-    const int lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5; // 32 pixel pairs x 8 rows, 2 rows per thread
-    const int x = x0 + 2 * lx2;
-    if (tf == 0)
-    { // every tile of this CTA is a copy tile: out = in, nothing staged
-#pragma unroll
-        for (int k = 0; k < THR / 8; k++)
-        {
-            const int y = y0 + lyb + 8 * k;
-            if (x >= W || y >= H || y >= P.row1) continue;
-            const size_t idx = (size_t)y * W + x;
-            if (x + 1 < W) *reinterpret_cast<uint4*>(out + idx) = __ldg(reinterpret_cast<const uint4*>(in + idx));
-            else out[idx] = __ldg(in + idx);
-        }
-        return;
-    }
-    for (int i = threadIdx.x; i < (RW / 2) * RH; i += 256)
-    {
-        const int rx = 2 * (i % (RW / 2)), ry = i / (RW / 2);
-        stage_pair9(g, in, P.c_sigma, x0 - PADL + rx, y0 - STEP + ry, W, H, ry * RW + rx, smem_f, PL);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < THR / 8; k++)
-    {
-        const int ly = lyb + 8 * k, y = y0 + ly;
-        if (x >= W || y >= H || y >= P.row1) continue;
-        const size_t idx  = (size_t)y * W + x;
-        const bool   has1 = x + 1 < W;
-        const int    ci   = (ly + STEP) * RW + 2 * lx2 + PADL;
-        int          k0 = 1, k1 = 1; // copy tile: pass-through
-        if ((tf >> ((ly >> 3) * 8 + (lx2 >> 2))) & 1u)
-        {
-            const float2 d  = has1 ? __ldg(reinterpret_cast<const float2*>(g.depth + idx)) : make_float2(__ldg(g.depth + idx), 1.0f);
-            const float  r0 = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx))).x;
-            const float  r1 = has1 ? h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx + 1))).x : 0.0f;
-            k0 = pixel_class(d.x, r0, P.approx);
-            k1 = has1 ? pixel_class(d.y, r1, P.approx) : 0;
-        }
-        float2 o_r = make_float2(0.f, 0.f), o_g = o_r, o_b = o_r, o_v = o_r, czs;
-        if (k0 == 2 || k1 == 2)
-        {
-            const float* s_va = smem_f + 7 * PL;
-            filter_pair<(STEP & 1) == 0>(smem_f, PL, ci, STEP * RW, STEP, s_va + ci - RW, s_va + ci + RW, P.c_phi0, o_r, o_g, o_b, o_v, czs);
-        }
-        store_pair(out, idx, has1, k0, k1, smem_f, PL, ci, o_r, o_g, o_b, o_v);
-    }
+    atrous_dense<ReflectionsPass, STEP>(g, in, tile_flags, P, out);
 }
 
-// Row-interleaved tile for the wide steps (see svgf_atrous_v3.cu::k_atrous_v3s): a CTA filters the 16 rows of one residue class
-// of the row index modulo STEP, so it stages 18 rows instead of 16 + 2 * STEP; the variance of the rows directly above / below
-// each filtered row (unit spacing, compute_variance_center) goes into two single-plane side buffers.
 template <int STEP>
 __global__ void __launch_bounds__(256) k_refl_atrous_v2s(GBufLevelDev g, const uint2* __restrict__ in, const uint8_t* __restrict__ tile_flags, R2Params P, uint2* __restrict__ out)
 {
-    extern __shared__ float smem_f[];
-    constexpr int PADL  = STEP; // STEP is even here
-    constexpr int RW    = TWR + 2 * STEP;
-    constexpr int RH    = THR + 2;
-    constexpr int PL    = RW * RH;
-    constexpr int TROWS = (THR * STEP) / 8; // 8-row tile rows spanned by the CTA's 16 * STEP image rows
-    float* s_vadj = smem_f + NPL * PL;      // [2][THR][RW]: variance of rows y-1 (0) and y+1 (1)
-    __shared__ uint8_t s_tfl[TROWS][8];
-    __shared__ int     s_any;
-    const int W = P.W, H = P.H;
-    const int x0 = blockIdx.x * TWR;
-    const int blk = blockIdx.y / STEP, phase = blockIdx.y - blk * STEP;
-    const int Y0 = P.row0 + blk * (THR * STEP); // multiple of 8 (row0 is)
-    const int TWt = (W + 7) >> 3, THt = (H + 7) >> 3;
-    if (threadIdx.x == 0) s_any = 0;
-    __syncthreads();
-    if (threadIdx.x < TROWS * 8)
-    {
-        const int  tx = (x0 >> 3) + (threadIdx.x & 7), ty = (Y0 >> 3) + (threadIdx.x >> 3);
-        const bool f  = tx < TWt && ty < THt && tile_flags[(size_t)ty * TWt + tx] != 0;
-        s_tfl[threadIdx.x >> 3][threadIdx.x & 7] = f ? 1 : 0;
-        if (f) s_any = 1;
-    }
-    __syncthreads();
-    const int lx2 = threadIdx.x & 31, lyb = threadIdx.x >> 5;
-    const int x = x0 + 2 * lx2;
-    if (!s_any)
-    {
-#pragma unroll
-        for (int k = 0; k < THR / 8; k++)
-        {
-            const int y = Y0 + phase + STEP * (lyb + 8 * k);
-            if (x >= W || y >= H || y >= P.row1) continue;
-            const size_t idx = (size_t)y * W + x;
-            if (x + 1 < W) *reinterpret_cast<uint4*>(out + idx) = __ldg(reinterpret_cast<const uint4*>(in + idx));
-            else out[idx] = __ldg(in + idx);
-        }
-        return;
-    }
-    for (int i = threadIdx.x; i < (RW / 2) * RH; i += 256)
-    {
-        const int rx = 2 * (i % (RW / 2)), ry = i / (RW / 2);
-        stage_pair9(g, in, P.c_sigma, x0 - PADL + rx, Y0 + phase + STEP * (ry - 1), W, H, ry * RW + rx, smem_f, PL);
-    }
-    constexpr int VP = TWR / 2 + 2; // texel pairs covering columns x0-2 .. x0+TWR+1
-    for (int i = threadIdx.x; i < 2 * THR * VP; i += 256)
-    {
-        const int a = i / (THR * VP), r = i - a * (THR * VP), j = r / VP, c = 2 * (r - j * VP);
-        const int px = x0 - 2 + c, py = Y0 + phase + STEP * j + (a ? 1 : -1);
-        float2    va = make_float2(0.0f, 0.0f);
-        if (px >= 0 && py >= 0 && px < W && py < H)
-        {
-            const uint4 w = __ldg(reinterpret_cast<const uint4*>(in + (size_t)py * W + px));
-            va = make_float2(h2_to_f2(w.y).y, h2_to_f2(w.w).y);
-        }
-        *reinterpret_cast<float2*>(s_vadj + (a * THR + j) * RW + PADL - 2 + c) = va;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < THR / 8; k++)
-    {
-        const int ly = lyb + 8 * k, y = Y0 + phase + STEP * ly;
-        if (x >= W || y >= H || y >= P.row1) continue;
-        const size_t idx  = (size_t)y * W + x;
-        const bool   has1 = x + 1 < W;
-        const int    ci   = (ly + 1) * RW + 2 * lx2 + PADL;
-        int          k0 = 1, k1 = 1;
-        if (s_tfl[(phase + STEP * ly) >> 3][lx2 >> 2])
-        {
-            const float2 d  = has1 ? __ldg(reinterpret_cast<const float2*>(g.depth + idx)) : make_float2(__ldg(g.depth + idx), 1.0f);
-            const float  r0 = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx))).x;
-            const float  r1 = has1 ? h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(g.gb3 + idx + 1))).x : 0.0f;
-            k0 = pixel_class(d.x, r0, P.approx);
-            k1 = has1 ? pixel_class(d.y, r1, P.approx) : 0;
-        }
-        float2 o_r = make_float2(0.f, 0.f), o_g = o_r, o_b = o_r, o_v = o_r, czs;
-        if (k0 == 2 || k1 == 2)
-            filter_pair<true>(smem_f, PL, ci, RW, STEP, s_vadj + (0 * THR + ly) * RW + 2 * lx2 + PADL, s_vadj + (1 * THR + ly) * RW + 2 * lx2 + PADL, P.c_phi0, o_r, o_g, o_b,
-                              o_v, czs);
-        store_pair(out, idx, has1, k0, k1, smem_f, PL, ci, o_r, o_g, o_b, o_v);
-    }
+    atrous_interleaved<ReflectionsPass, STEP>(g, in, tile_flags, P, out);
 }
-
-template <int STEP>
-void launch_r2(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, cudaStream_t st)
-{
-    constexpr int PADL = STEP + (STEP & 1);
-    constexpr int RW   = (TWR + PADL + STEP + 1) & ~1;
-    constexpr int RH   = THR + 2 * STEP;
-    const size_t  smem = (size_t)RW * RH * NPL * sizeof(float);
-    static bool   configured[64] = {};
-    if (hr_once_per_device(configured)) cudaFuncSetAttribute(k_refl_atrous_v2<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    dim3 grid((P.W + TWR - 1) / TWR, (P.row1 - P.row0 + THR - 1) / THR);
-    k_refl_atrous_v2<STEP><<<grid, 256, smem, st>>>(g, in, tf, P, out);
-}
-
-template <int STEP>
-void launch_r2s(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, const R2Params& P, uint2* out, cudaStream_t st)
-{
-    constexpr int RW = TWR + 2 * STEP, RH = THR + 2;
-    const size_t  smem = ((size_t)RW * RH * NPL + (size_t)2 * THR * RW) * sizeof(float);
-    static bool   configured[64] = {};
-    if (hr_once_per_device(configured)) cudaFuncSetAttribute(k_refl_atrous_v2s<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    const int rows = P.row1 - P.row0, blocks = (rows + THR * STEP - 1) / (THR * STEP);
-    dim3      grid((P.W + TWR - 1) / TWR, blocks * STEP);
-    k_refl_atrous_v2s<STEP><<<grid, 256, smem, st>>>(g, in, tf, P, out);
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // TMA-staged, persistent form of the dense-tile kernel at step 1.
@@ -386,15 +154,10 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, ui
                  : "memory");
 }
 
-// the region of k_refl_atrous_v2<1>
-struct TmaGeom {
-    static constexpr int STEP = 1;
-    static constexpr int PADL = STEP + (STEP & 1);
-    static constexpr int RW   = (TWR + PADL + STEP + 1) & ~1;
-    static constexpr int RH   = THR + 2 * STEP;
-    static constexpr int PL   = RW * RH;
-    static constexpr int RAWB = (PL * 8 + 127) & ~127; // bytes of one raw image box, padded to the 128-byte TMA destination alignment
-    static constexpr int SMEM = 3 * RAWB + NPL * PL * 4 + TWR * THR; // + one class byte per pixel of the tile
+// the region of k_refl_atrous_v2<1>; shared memory: three raw image boxes of it, the planes, one class byte per pixel of the tile
+struct TmaGeom : DenseTile<1, ReflectionsPass::NPL> {
+    static constexpr int RAWB  = (PL * 8 + 127) & ~127; // bytes of one raw image box, padded to the 128-byte TMA destination alignment
+    static constexpr int BYTES = 3 * RAWB + SMEM + PAIR_TILE_W * PAIR_TILE_H;
 };
 
 __global__ void __launch_bounds__(256, 3)
@@ -403,11 +166,11 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
                   unsigned int* __restrict__ counter)
 {
     using G = TmaGeom;
-    constexpr int STEP = G::STEP, PADL = G::PADL, RW = G::RW, RH = G::RH, PL = G::PL;
+    constexpr int STEP = 1, PADL = G::PADL, RW = G::RW, RH = G::RH, PL = G::PL;
     extern __shared__ __align__(128) unsigned char smem_b[];
     unsigned char* raw0 = smem_b;
     float*         planes = reinterpret_cast<float*>(smem_b + 3 * G::RAWB);
-    unsigned char* s_cls  = smem_b + 3 * G::RAWB + NPL * PL * 4; // per pixel of the tile: 0 sky, 1 pass-through, 2 filter (pixel_class)
+    unsigned char* s_cls  = smem_b + 3 * G::RAWB + G::SMEM; // per pixel of the tile: 0 sky, 1 pass-through, 2 filter (pixel_class)
     __shared__ __align__(8) uint64_t s_mbar;
     __shared__ int      s_tile[2];
     __shared__ uint32_t s_flag[2];
@@ -424,7 +187,7 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
         bool f = false;
         if (t < n_tiles && lane < 16)
         {
-            const int x0 = (t % tiles_x) * TWR, y0 = P.row0 + (t / tiles_x) * THR;
+            const int x0 = (t % tiles_x) * PAIR_TILE_W, y0 = P.row0 + (t / tiles_x) * PAIR_TILE_H;
             const int tx = (x0 >> 3) + (lane & 7), ty = (y0 >> 3) + (lane >> 3);
             f = tx < TWt && ty < THt && tile_flags[(size_t)ty * TWt + tx] != 0;
         }
@@ -432,7 +195,7 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
         if (lane == 0) { s_tile[slot] = t < n_tiles ? t : -1; s_flag[slot] = b; }
     };
     auto issue_tma = [&](int t) { // one thread
-        const int x0 = (t % tiles_x) * TWR, y0 = P.row0 + (t / tiles_x) * THR;
+        const int x0 = (t % tiles_x) * PAIR_TILE_W, y0 = P.row0 + (t / tiles_x) * PAIR_TILE_H;
         mbar_arrive_expect_tx(&s_mbar, 3u * (uint32_t)(PL * 8));
         tma_load_2d(raw0, &tm_gb2, &s_mbar, x0 - PADL, y0 - STEP);
         tma_load_2d(raw0 + G::RAWB, &tm_gb3, &s_mbar, x0 - PADL, y0 - STEP);
@@ -451,7 +214,7 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
         const uint32_t tf = s_flag[slot];
         if (t < 0) break;
         if (warp == 0) fetch_tile(slot ^ 1); // overlaps the wait below
-        const int x0 = (t % tiles_x) * TWR, y0 = P.row0 + (t / tiles_x) * THR;
+        const int x0 = (t % tiles_x) * PAIR_TILE_W, y0 = P.row0 + (t / tiles_x) * PAIR_TILE_H;
         if (tf != 0u)
         {
             {
@@ -493,12 +256,12 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
                 *reinterpret_cast<float2*>(p) = va; p += PL;
                 *reinterpret_cast<float2*>(p) = lu;
                 const int tx = rx - PADL, ty = ry - STEP;
-                if (tx >= 0 && tx < TWR && ty >= 0 && ty < THR)
+                if (tx >= 0 && tx < PAIR_TILE_W && ty >= 0 && ty < PAIR_TILE_H)
                 { // the reference's early-outs (:119-128).  Sky = linear z < 0 (GB3.w = -1): identical to its depth == 1 test whenever the
                   // sky pixels carry the G-buffer clear values (depth 1 and GB3 = (0,0,0,-1) are written together, g_buffer.cpp:72-96)
                     const int c0 = zs.x < 0.0f ? 0 : ((rough.x < 0.05f || (P.approx == 1 && rough.x > 0.75f)) ? 1 : 2);
                     const int c1 = zs.y < 0.0f ? 0 : ((rough.y < 0.05f || (P.approx == 1 && rough.y > 0.75f)) ? 1 : 2);
-                    *reinterpret_cast<uchar2*>(s_cls + ty * TWR + tx) = make_uchar2((unsigned char)c0, (unsigned char)c1);
+                    *reinterpret_cast<uchar2*>(s_cls + ty * PAIR_TILE_W + tx) = make_uchar2((unsigned char)c0, (unsigned char)c1);
                 }
             }
         }
@@ -510,7 +273,7 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
         }
         const int x = x0 + 2 * lx2;
 #pragma unroll
-        for (int k = 0; k < THR / 8; k++)
+        for (int k = 0; k < PAIR_TILE_H / 8; k++)
         {
             const int ly = lyb + 8 * k, y = y0 + ly;
             if (x >= W || y >= H || y >= P.row1) continue;
@@ -522,19 +285,19 @@ k_refl_atrous_tma(const __grid_constant__ CUtensorMap tm_gb2, const __grid_const
             }
             const int ci = (ly + STEP) * RW + 2 * lx2 + PADL;
             int       k0 = 1, k1 = 1;
-            if ((tf >> ((ly >> 3) * 8 + (lx2 >> 2))) & 1u)
+            if ((tf >> dense_flag_bit(lx2, ly)) & 1u)
             {
-                const uchar2 c = *reinterpret_cast<const uchar2*>(s_cls + ly * TWR + 2 * lx2);
+                const uchar2 c = *reinterpret_cast<const uchar2*>(s_cls + ly * PAIR_TILE_W + 2 * lx2);
                 k0 = c.x;
                 k1 = c.y;
             }
-            float2 o_r = make_float2(0.f, 0.f), o_g = o_r, o_b = o_r, o_v = o_r, czs;
+            PairSum<3> f = {};
             if (k0 == 2 || k1 == 2)
             {
                 const float* s_va = planes + 7 * PL;
-                filter_pair<(STEP & 1) == 0>(planes, PL, ci, STEP * RW, STEP, s_va + ci - RW, s_va + ci + RW, P.c_phi0, o_r, o_g, o_b, o_v, czs);
+                f = filter_pair<3, 8, (STEP & 1) == 0>(PairTaps { planes, PL, ci, STEP * RW, STEP, s_va + ci - RW, s_va + ci + RW }, P.c_phi0);
             }
-            store_pair(out, idx, true, k0, k1, planes, PL, ci, o_r, o_g, o_b, o_v);
+            store_pair(out, idx, true, k0, k1, planes, PL, ci, f);
         }
         __syncthreads(); // planes may be overwritten by the next tile's decode
         slot ^= 1;
@@ -595,18 +358,23 @@ bool launch_r2_tma(const GBufLevelDev& g, const uint2* in, const uint8_t* tf, co
     static bool configured[64] = {};
     if (hr_once_per_device(configured))
     {
-        cudaFuncSetAttribute(k_refl_atrous_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM);
+        cudaFuncSetAttribute(k_refl_atrous_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BYTES);
         int sms = 132, per_sm = 1;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_atrous_tma, 256, G::SMEM);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refl_atrous_tma, 256, G::BYTES);
         ctas[dev] = sms * (per_sm > 0 ? per_sm : 1);
     }
-    const int tiles_x = (P.W + TWR - 1) / TWR, tiles_y = (P.row1 - P.row0 + THR - 1) / THR, n_tiles = tiles_x * tiles_y;
+    const int tiles_x = (P.W + PAIR_TILE_W - 1) / PAIR_TILE_W, tiles_y = (P.row1 - P.row0 + PAIR_TILE_H - 1) / PAIR_TILE_H, n_tiles = tiles_x * tiles_y;
     cudaMemsetAsync(counter, 0, sizeof(unsigned int), st);
     const int grid = ctas[dev] < n_tiles ? ctas[dev] : n_tiles;
-    k_refl_atrous_tma<<<grid, 256, G::SMEM, st>>>(t2, t3, ti, g, in, tf, P, out, tiles_x, n_tiles, counter);
+    k_refl_atrous_tma<<<grid, 256, G::BYTES, st>>>(t2, t3, ti, g, in, tf, P, out, tiles_x, n_tiles, counter);
     return true;
 }
+
+template <int STEP>
+using Dense = DenseTile<STEP, ReflectionsPass::NPL>;
+template <int STEP>
+using Interleaved = InterleavedTile<STEP, ReflectionsPass::NPL>;
 
 } // namespace
 
@@ -628,11 +396,13 @@ bool launch_reflections_atrous_v2(const GBufLevelDev& g, const void* in, const u
     uint2*       o2 = (uint2*)out;
     switch (step)
     {
-        case 1: if (!(g_hr_refl_atrous_impl == 3 && launch_r2_tma(g, i2, tile_flags, P, o2, counters, st))) launch_r2<1>(g, i2, tile_flags, P, o2, st); break;
-        case 2: launch_r2<2>(g, i2, tile_flags, P, o2, st); break;
-        case 4: launch_r2<4>(g, i2, tile_flags, P, o2, st); break;
-        case 8: launch_r2s<8>(g, i2, tile_flags, P, o2, st); break;
-        default: launch_r2s<16>(g, i2, tile_flags, P, o2, st); break;
+        case 1:
+            if (!(g_hr_refl_atrous_impl == 3 && launch_r2_tma(g, i2, tile_flags, P, o2, counters, st))) launch_tiles<Dense<1>>(k_refl_atrous_v2<1>, g, i2, tile_flags, P, o2, st);
+            break;
+        case 2: launch_tiles<Dense<2>>(k_refl_atrous_v2<2>, g, i2, tile_flags, P, o2, st); break;
+        case 4: launch_tiles<Dense<4>>(k_refl_atrous_v2<4>, g, i2, tile_flags, P, o2, st); break;
+        case 8: launch_tiles<Interleaved<8>>(k_refl_atrous_v2s<8>, g, i2, tile_flags, P, o2, st); break;
+        default: launch_tiles<Interleaved<16>>(k_refl_atrous_v2s<16>, g, i2, tile_flags, P, o2, st); break;
     }
     return true;
 }

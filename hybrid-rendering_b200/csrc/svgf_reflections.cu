@@ -422,9 +422,6 @@ void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& pr
     else k_refl_temporal<false><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
 }
 
-bool launch_reflections_atrous_v2(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
-                                  float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st); // svgf_refl_atrous_v2.cu
-
 int launch_reflections_atrous(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
                               float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st)
 {
