@@ -88,6 +88,34 @@ class hr_pass_stats(C.Structure):
                 ("pixels_total", C.c_uint64), ("renders", C.c_uint64)]
 
 
+class hr_compare_params(C.Structure):
+    _fields_ = [("relmse_eps", C.c_float), ("ssim_c1", C.c_float), ("ssim_c2", C.c_float)]
+
+
+class hr_compare_sums(C.Structure):
+    """integer sums of hr_image_compare; the 128-bit fields as Python integers: sq(), abs(), rel() unsigned, ssim_sum() signed"""
+    _fields_ = [("pixels", C.c_uint64), ("nonfinite_test", C.c_uint64), ("nonfinite_ref", C.c_uint64), ("sq_err", C.c_uint64 * 2),
+                ("abs_err", C.c_uint64 * 2), ("rel_err", C.c_uint64 * 2), ("ssim", C.c_uint64 * 2), ("max_abs_err", C.c_uint32), ("_pad", C.c_uint32)]
+
+    def sq(self):
+        return self.sq_err[0] | (self.sq_err[1] << 64)
+
+    def abs(self):
+        return self.abs_err[0] | (self.abs_err[1] << 64)
+
+    def rel(self):
+        return self.rel_err[0] | (self.rel_err[1] << 64)
+
+    def ssim_sum(self):
+        v = self.ssim[0] | (self.ssim[1] << 64)
+        return v - (1 << 128) if v >> 127 else v
+
+
+class hr_compare_result(C.Structure):
+    _fields_ = [("mse", C.c_double), ("rmse", C.c_double), ("psnr", C.c_double), ("relmse", C.c_double), ("mean_abs", C.c_double), ("max_abs", C.c_double),
+                ("ssim", C.c_double), ("pixels", C.c_uint64), ("nonfinite_test", C.c_uint64), ("nonfinite_ref", C.c_uint64)]
+
+
 class hrs_light_desc(C.Structure):
     _fields_ = [("type", C.c_int32), ("rot_y_deg", C.c_float), ("rot_x_deg", C.c_float), ("position", C.c_float * 3), ("radius", C.c_float),
                 ("intensity", C.c_float), ("color", C.c_float * 3), ("cone_inner_deg", C.c_float), ("cone_outer_deg", C.c_float)]
@@ -106,6 +134,7 @@ ABI_SYMBOLS = [
     "hr_ddgi_default_params", "hr_ddgi_create", "hr_ddgi_render", "hr_ddgi_get_uniforms", "hr_reflections_default_params", "hr_reflections_create",
     "hr_reflections_render", "hr_pass_get_stats", "hr_pass_output_checksum", "hr_gbuffer_render", "hr_gbuffer_render_sharded", "hr_brdf_lut_set", "hr_deferred_create", "hr_deferred_render", "hr_gbuffer_stage_render", "hr_bluenoise_set_slot",
     "hr_taa_default_params", "hr_taa_jitter", "hr_taa_create", "hr_taa_render", "hr_tonemap_default_params", "hr_tonemap_create", "hr_tonemap_render", "hr_path_tracer_default_params", "hr_path_tracer_create", "hr_path_tracer_render", "hr_scene_set_textures",
+    "hr_compare_default_params", "hr_compare_sums_add", "hr_compare_finish", "hr_image_compare",
 ]
 
 _product = None
@@ -183,6 +212,25 @@ def shard_rows(H, rank, world):
 
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def compare_default_params():
+    p = hr_compare_params()
+    load_product().hr_compare_default_params(C.byref(p))
+    return p
+
+
+def sums_add(acc: hr_compare_sums, s: hr_compare_sums):
+    """hr_compare_sums_add: acc += s (pure host function); returns acc"""
+    load_product().hr_compare_sums_add(C.byref(acc), C.byref(s))
+    return acc
+
+
+def compare_finish(s: hr_compare_sums):
+    """hr_compare_finish: mse, rmse, psnr, relmse, mean_abs, max_abs, ssim of the sums (pure host function)"""
+    r = hr_compare_result()
+    load_product().hr_compare_finish(C.byref(s), C.byref(r))
+    return r
 
 
 # ---------------------------------------------------------------------------------------------- synthetic inputs
@@ -459,6 +507,17 @@ class Context:
 
     def launch_count(self):
         return int(self.lib.hr_ctx_launch_count(self.h))
+
+    def compare(self, test, ref, row0=0, row1=0, error_map=None, params=None, stream=0):
+        """hr_image_compare of `test` against `ref` over rows [row0, row1) (row1 <= 0: the whole image) -> hr_compare_sums.  test, ref: hr_image
+        values or passes (their final output, which = 100); error_map: an RGBA16F hr_image of their size, or None; params: hr_compare_params
+        (None: the defaults)"""
+        t, r = [x.output(100) if isinstance(x, Pass) else x for x in (test, ref)]
+        out = hr_compare_sums()
+        p = params if params is not None else compare_default_params()
+        self.check(self.lib.hr_image_compare(self.h, C.byref(t), C.byref(r), C.byref(p), row0, row1, C.byref(out),
+                                             C.byref(error_map) if error_map is not None else None, C.c_void_p(stream)), "hr_image_compare")
+        return out
 
     def set_profiling(self, on):
         self.lib.hr_ctx_set_profiling(self.h, int(on))

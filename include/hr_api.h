@@ -596,6 +596,59 @@ HR_API int hr_pass_get_stats(hr_pass* pass, hr_pass_stats* out, void* stream);
 HR_API int hr_pass_output_checksum(hr_pass* pass, int which, int row0, int row1, uint64_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Image comparison (not in the reference, whose judge is a person flipping between the "Ground Truth" view and the hybrid frame):
+ * error sums and SSIM of a test image against a reference image, e.g. the deferred combine's FINAL output against the path tracer's,
+ * computed on the device.  The per-pixel terms are bit-specified (DESIGN.md §5, restated in tests/image_compare.py):
+ *   t, r = the pixel's C channels as float (RGBA16F and RGBA8: rgb, alpha ignored, RGBA8 as b / 255; RG16F: r, g; R16F: r); d = t - r;
+ *   se = (sum d^2) / C,  ae = (sum |d|) / C,  rel = (sum d^2 / (r^2 + relmse_eps)) / C, each channel sum in channel order;
+ *   a pixel with a NaN or infinite channel in t (r) counts in nonfinite_test (nonfinite_ref) and is left out of every sum;
+ *   luminance Y = (0.299 c0 + 0.587 c1) + 0.114 c2 of the channels clamped to [0, 1] (one channel: clamp(c0); two: c2 = 0), 0 in both
+ *   images at a left-out pixel; SSIM over the 11-tap Gaussian window (sigma 1.5, float weights of the normalised double Gaussian),
+ *   rows first, then columns, taps clamped to the image:
+ *   ssim = ((2 mu_t mu_r + ssim_c1)(2 cov + ssim_c2)) / ((mu_t^2 + mu_r^2 + ssim_c1)(var_t + var_r + ssim_c2)).
+ * Each term x enters its sum as round-to-nearest-even(x * 2^32), x clamped to [-2^63, 2^63] (NaN, possible only with zero
+ * parameters: 0).  The sums are integers, so they do not depend on the launch and the sums of any row split (one per rank of a
+ * sharded run) add up to the whole image's.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct hr_compare_params {
+    float relmse_eps; /* 0.01: relMSE term d^2 / (r^2 + eps) */
+    float ssim_c1;    /* 1e-4 = (0.01 * 1)^2 */
+    float ssim_c2;    /* 9e-4 = (0.03 * 1)^2 */
+} hr_compare_params;
+HR_API void hr_compare_default_params(hr_compare_params* p);
+
+typedef struct hr_compare_sums {   /* integers: order-independent; the sums of any row split add up to the whole image's */
+    uint64_t pixels;               /* pixels summed (both texels finite)                                                  */
+    uint64_t nonfinite_test, nonfinite_ref;
+    uint64_t sq_err[2], abs_err[2], rel_err[2]; /* unsigned 128-bit (lo, hi), fixed point 2^-32                           */
+    uint64_t ssim[2];              /* signed 128-bit two's complement, fixed point 2^-32                                  */
+    uint32_t max_abs_err;          /* float bits of the largest per-pixel channel |d| (max of non-negative floats = max of their bits) */
+    uint32_t _pad;
+} hr_compare_sums;
+/* Pure: acc += s (128-bit adds wrapping mod 2^128, counts added, max_abs_err the larger). */
+HR_API void hr_compare_sums_add(hr_compare_sums* acc, const hr_compare_sums* s);
+
+typedef struct hr_compare_result {
+    double   mse, rmse, psnr, relmse, mean_abs, max_abs, ssim;
+    uint64_t pixels, nonfinite_test, nonfinite_ref;
+} hr_compare_result;
+/* Pure: the means of the sums, each (double)(sum) * 2^-32 / (double)pixels (the 128-bit integer rounded once to double); rmse =
+ * sqrt(mse); psnr = 10 log10(1 / mse), +inf at mse 0; max_abs = the float of max_abs_err.  No pixel summed: the means are NaN. */
+HR_API void hr_compare_finish(const hr_compare_sums* s, hr_compare_result* out);
+
+/* test, ref: device images of equal size and format (hr_pass_output of two passes, or caller memory).  Rows [row0, row1) are summed
+ * (row1 <= 0 = whole image; any other range outside [0, height] or with row1 < row0 returns HR_ERR_INVALID_ARG).  SSIM windows read
+ * 5 rows beyond the range (clamped to the image), so those rows must be valid: gathered FINAL outputs are.  error_map: optional caller
+ * device RGBA16F W x H image that receives (ae, se, rel, ssim) rounded to fp16 for the pixels of the range's rows (a left-out pixel:
+ * four quiet NaNs, 0x7E00); its other rows are not written.  R32_UINT and R8_UINT images return HR_ERR_UNSUPPORTED; a size or format
+ * mismatch, a NULL argument, a bad row range, an error map of another size or format or whose bytes overlap test's or ref's, or a negative
+ * or non-finite parameter returns
+ * HR_ERR_INVALID_ARG.  A refused call writes nothing to `out` or `error_map`.  Two kernels (per-tile sums, then their total; none for
+ * an empty range).  Synchronises `stream`. */
+HR_API int hr_image_compare(hr_ctx* ctx, const hr_image* test, const hr_image* ref, const hr_compare_params* params, int row0, int row1,
+                            hr_compare_sums* out, hr_image* error_map, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Screen-space row-band sharding across GPUs (new; SURVEY.md §8e).  rank owns pass rows
  * [row_begin, row_end) aligned to 8; the other rows are skipped by every stage except a halo.
  * ---------------------------------------------------------------------------------------------- */
