@@ -21,6 +21,8 @@
 // Internal node ids are handed out downwards from n-2 so that the last merge (the root) is node 0; after the tree is
 // complete every leaf walks to the root to find its depth-first position, which makes the triangles of every subtree
 // contiguous again (needed for the <= LEAF_MAX leaf collapse) and gives the (first,last) range of every node.
+// Before that, g_hr_bvh_treelet_rounds (3) rounds of treelet restructuring (k_treelet) lower the tree's SAH cost; the
+// depth-first order and the leaf ranges are computed on the final topology.
 //
 // Node layout (4 x float4):  n0 = (c0.lo.x, c0.hi.x, c0.lo.y, c0.hi.y)   n1 = (c1.lo.x, c1.hi.x, c1.lo.y, c1.hi.y)
 //                            nz = (c0.lo.z, c0.hi.z, c1.lo.z, c1.hi.z)   ch = (int c0, int c1, -, -) as bits
@@ -196,18 +198,19 @@ __device__ __forceinline__ float box_pad(const int* __restrict__ bounds)
     return ext * (1.0f / 65536.0f) + mag * (1.0f / 1048576.0f) + 1e-7f;
 }
 
-__device__ __forceinline__ int encode_child(int ch, int n, const int2* __restrict__ ranges)
+// A subtree of <= LEAF_MAX triangles becomes one leaf; as_leaf (null: always) is the treelet optimiser's choice per node.
+__device__ __forceinline__ int encode_child(int ch, int n, const int2* __restrict__ ranges, const int* __restrict__ as_leaf)
 {
     if (ch >= n - 1) return ~(((ch - (n - 1)) << 3) | 0);
     int2 r = ranges[ch];
     int  cnt = r.y - r.x + 1;
-    if (cnt <= LEAF_MAX) return ~((r.x << 3) | (cnt - 1));
+    if (cnt <= LEAF_MAX && (!as_leaf || as_leaf[ch])) return ~((r.x << 3) | (cnt - 1));
     return ch;
 }
 
-__global__ void k_pack_nodes(int n, const int2* __restrict__ children, const int2* __restrict__ ranges, const float* __restrict__ tri_aabb,
-                             const uint32_t* __restrict__ sorted_prim, const float* __restrict__ node_aabb, const int* __restrict__ bounds,
-                             float4* __restrict__ out)
+__global__ void k_pack_nodes(int n, const int2* __restrict__ children, const int2* __restrict__ ranges, const int* __restrict__ as_leaf,
+                             const float* __restrict__ tri_aabb, const uint32_t* __restrict__ sorted_prim, const float* __restrict__ node_aabb,
+                             const int* __restrict__ bounds, float4* __restrict__ out)
 {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n - 1) return;
@@ -227,7 +230,7 @@ __global__ void k_pack_nodes(int n, const int2* __restrict__ children, const int
     out[4ull * i + 0] = make_float4(b[0][0], b[0][3], b[0][1], b[0][4]);
     out[4ull * i + 1] = make_float4(b[1][0], b[1][3], b[1][1], b[1][4]);
     out[4ull * i + 2] = make_float4(b[0][2], b[0][5], b[1][2], b[1][5]);
-    out[4ull * i + 3] = make_float4(__int_as_float(encode_child(c.x, n, ranges)), __int_as_float(encode_child(c.y, n, ranges)), 0.0f, 0.0f);
+    out[4ull * i + 3] = make_float4(__int_as_float(encode_child(c.x, n, ranges, as_leaf)), __int_as_float(encode_child(c.y, n, ranges, as_leaf)), 0.0f, 0.0f);
 }
 
 // n <= LEAF_MAX (or n == 1): a single node whose child 0 is the leaf [0,n) with the scene box, child 1 is empty.
@@ -400,15 +403,260 @@ __global__ void k_ploc_remap(int n, int2* __restrict__ children, const int* __re
     children[i] = c;
 }
 
+// ---- treelet restructuring (Karras & Aila 2013, "Fast Parallel Construction of High-Quality BVHs") ----------------------
+// PLOC clusters within +-PLOC_R slots of the Morton order, which leaves poor splits in the upper levels of long planar scenes.
+// Every round walks the binary tree bottom-up (the k_fit flag pattern: the second arrival at a node owns it, and its whole
+// subtree is final).  At each node one warp grows a treelet of up to TREELET_LEAVES leaves by repeatedly opening the treelet
+// leaf of largest area, finds the topology of least SAH cost over those leaves by dynamic programming over their subsets, and
+// rewires the treelet's internal nodes (same ids, new children, refitted boxes) when that is cheaper.
+//
+// Cost model of the traversal (per ray, in issued instructions): a node step tests both child boxes (~75), a triangle test
+// ~80.  SAH(node) = SAH_CI * A(node) + SAH(children), a leaf of c triangles costs SAH_CT * c * A(leaf); a subtree of
+// <= LEAF_MAX triangles is packed as one leaf when that is cheaper (as_leaf), which k_pack_nodes follows.
+// A treelet whose new height would take a triangle deeper than max_depth keeps its input topology: depth[] holds every
+// internal node's depth at the start of the round, and a node's ancestors are restructured only after it.
+#define TREELET_LEAVES 7
+#define TREELET_WARPS  4
+#define SAH_CI 75.0f
+#define SAH_CT 80.0f
+
+struct Treelet
+{
+    int           leaf[TREELET_LEAVES], size[TREELET_LEAVES], height[TREELET_LEAVES], inner[TREELET_LEAVES - 1];
+    float         box[TREELET_LEAVES][6], cost[TREELET_LEAVES];
+    float         area[1 << TREELET_LEAVES], sah[1 << TREELET_LEAVES];
+    unsigned char part[1 << TREELET_LEAVES], as_leaf[1 << TREELET_LEAVES];
+};
+
+__device__ __forceinline__ float half_area(const float* b)
+{
+    const float dx = b[3] - b[0], dy = b[4] - b[1], dz = b[5] - b[2];
+    return dx * dy + dy * dz + dz * dx;
+}
+
+// box, triangle count, SAH cost and height of a node or triangle (ids >= n-1); written earlier in this kernel, hence L2 loads
+__device__ __forceinline__ void treelet_leaf(Treelet& t, int slot, int id, int n, const float* __restrict__ tri_aabb, const uint32_t* __restrict__ prim,
+                                             const float* node_aabb, const int* sizes, const float* cost, const int* height)
+{
+    const bool   tri = id >= n - 1;
+    const float* b   = tri ? tri_aabb + 6ull * prim[id - (n - 1)] : node_aabb + 6ull * id;
+    for (int a = 0; a < 6; a++) t.box[slot][a] = __ldcg(b + a);
+    t.leaf[slot]   = id;
+    t.size[slot]   = tri ? 1 : __ldcg(sizes + id);
+    t.cost[slot]   = tri ? SAH_CT * half_area(t.box[slot]) : __ldcg(cost + id);
+    t.height[slot] = tri ? 0 : __ldcg(height + id);
+}
+
+__device__ void treelet_node(Treelet& t, int root, int n, const float* __restrict__ tri_aabb, const uint32_t* __restrict__ prim, int2* children,
+                             int* parent, float* node_aabb, int* sizes, float* cost, int* height, int* as_leaf, const int* __restrict__ depth, int max_depth)
+{
+    const unsigned FULL = 0xFFFFFFFFu;
+    const int      lane = threadIdx.x & 31;
+    int            L    = 0;
+    if (lane == 0)
+    {
+        const int2 c = __ldcg(children + root);
+        treelet_leaf(t, 0, c.x, n, tri_aabb, prim, node_aabb, sizes, cost, height);
+        treelet_leaf(t, 1, c.y, n, tri_aabb, prim, node_aabb, sizes, cost, height);
+        t.inner[0] = root;
+        for (L = 2; L < TREELET_LEAVES; L++)
+        {
+            int   open = -1;
+            float best = -1.0f;
+            for (int i = 0; i < L; i++)
+                if (t.leaf[i] < n - 1 && half_area(t.box[i]) > best) { best = half_area(t.box[i]); open = i; }
+            if (open < 0) break;
+            const int2 oc = __ldcg(children + t.leaf[open]);
+            t.inner[L - 1] = t.leaf[open];
+            treelet_leaf(t, open, oc.x, n, tri_aabb, prim, node_aabb, sizes, cost, height);
+            treelet_leaf(t, L, oc.y, n, tri_aabb, prim, node_aabb, sizes, cost, height);
+        }
+    }
+    L = __shfl_sync(FULL, L, 0);
+    __syncwarp();
+    const unsigned full = (1u << L) - 1;
+    // areas of all subsets; singletons cost what their subtree costs, larger subsets start from the one-leaf option
+    for (unsigned m = 1 + lane; m <= full; m += 32)
+    {
+        float b[6] = { FLT_MAX, FLT_MAX, FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX };
+        int   sz   = 0;
+        for (int i = 0; i < L; i++)
+            if (m >> i & 1)
+            {
+                for (int a = 0; a < 3; a++) { b[a] = fminf(b[a], t.box[i][a]); b[3 + a] = fmaxf(b[3 + a], t.box[i][3 + a]); }
+                sz += t.size[i];
+            }
+        t.area[m] = half_area(b);
+        t.sah[m]  = __popc(m) == 1 ? t.cost[__ffs(m) - 1] : sz <= LEAF_MAX ? SAH_CT * (float)sz * t.area[m] : FLT_MAX;
+    }
+    __syncwarp();
+    // subsets by size: the best split of m into p (holding m's lowest leaf) and m ^ p
+    for (int k = 2; k <= L; k++)
+    {
+        for (unsigned m = 1 + lane; m <= full; m += 32)
+        {
+            if (__popc(m) != k) continue;
+            const unsigned low = m & (0u - m), rest = m ^ low;
+            float          best = FLT_MAX;
+            unsigned       bp   = low;
+            unsigned       q    = rest;
+            do
+            {
+                q = (q - 1) & rest;
+                const unsigned p = low | q;
+                const float    c = t.sah[p] + t.sah[m ^ p];
+                if (c < best) { best = c; bp = p; }
+            } while (q);
+            const float inner = SAH_CI * t.area[m] + best, leafc = t.sah[m];
+            t.part[m]    = (unsigned char)bp;
+            t.as_leaf[m] = leafc <= inner;
+            t.sah[m]     = fminf(leafc, inner);
+        }
+        __syncwarp();
+    }
+    if (lane == 0)
+    {
+        // the input topology's cost, from the root's children
+        const int2  c     = __ldcg(children + root);
+        float       cc[2];
+        int         hh[2];
+        for (int s = 0; s < 2; s++)
+        {
+            const int ch = s ? c.y : c.x;
+            if (ch >= n - 1)
+            {
+                const float* b = tri_aabb + 6ull * prim[ch - (n - 1)];
+                float        bb[6];
+                for (int a = 0; a < 6; a++) bb[a] = b[a];
+                cc[s] = SAH_CT * half_area(bb);
+                hh[s] = 0;
+            }
+            else { cc[s] = __ldcg(cost + ch); hh[s] = __ldcg(height + ch); }
+        }
+        const int   sz    = __ldcg(sizes + root);
+        const float inner = SAH_CI * t.area[full] + cc[0] + cc[1], leafc = sz <= LEAF_MAX ? SAH_CT * (float)sz * t.area[full] : FLT_MAX;
+        float       old_c = fminf(inner, leafc);
+        int         old_h = 1 + max(hh[0], hh[1]);
+        bool        keep  = true;
+        if (L > 2 && t.sah[full] < old_c * (1.0f - 1e-5f))
+        {
+            // new internal nodes in pre-order (root first); ref >= 0: internal node ord, < 0: treelet leaf ~ref
+            unsigned om[TREELET_LEAVES - 1];
+            int      ref[TREELET_LEAVES - 1][2], nh[TREELET_LEAVES - 1];
+            int      cnt = 1;
+            om[0]        = full;
+            for (int i = 0; i < cnt; i++)
+                for (int s = 0; s < 2; s++)
+                {
+                    const unsigned side = s ? om[i] ^ t.part[om[i]] : t.part[om[i]];
+                    if (__popc(side) == 1) ref[i][s] = ~(__ffs(side) - 1);
+                    else { ref[i][s] = cnt; om[cnt++] = side; }
+                }
+            for (int i = cnt - 1; i >= 0; i--)
+            {
+                const int h0 = ref[i][0] >= 0 ? nh[ref[i][0]] : t.height[~ref[i][0]];
+                const int h1 = ref[i][1] >= 0 ? nh[ref[i][1]] : t.height[~ref[i][1]];
+                nh[i]        = 1 + max(h0, h1);
+            }
+            if (nh[0] <= max_depth - __ldcg(depth + root))
+            {
+                keep = false;
+                for (int i = 0; i < cnt; i++)
+                {
+                    const int id = t.inner[i];
+                    int       ids[2];
+                    for (int s = 0; s < 2; s++) ids[s] = ref[i][s] >= 0 ? t.inner[ref[i][s]] : t.leaf[~ref[i][s]];
+                    float b[6] = { FLT_MAX, FLT_MAX, FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX };
+                    int   nsz  = 0;
+                    for (int j = 0; j < L; j++)
+                        if (om[i] >> j & 1)
+                        {
+                            for (int a = 0; a < 3; a++) { b[a] = fminf(b[a], t.box[j][a]); b[3 + a] = fmaxf(b[3 + a], t.box[j][3 + a]); }
+                            nsz += t.size[j];
+                        }
+                    __stcg(children + id, make_int2(ids[0], ids[1]));
+                    __stcg(parent + ids[0], id);
+                    __stcg(parent + ids[1], id);
+                    for (int a = 0; a < 6; a++) __stcg(node_aabb + 6ull * id + a, b[a]);
+                    __stcg(sizes + id, nsz);
+                    __stcg(cost + id, t.sah[om[i]]);
+                    __stcg(height + id, nh[i]);
+                    __stcg(as_leaf + id, (int)t.as_leaf[om[i]]);
+                }
+            }
+        }
+        if (keep)
+        {
+            __stcg(cost + root, old_c);
+            __stcg(height + root, old_h);
+            __stcg(as_leaf + root, (int)(leafc <= inner));
+        }
+        __threadfence();
+    }
+    __syncwarp();
+}
+
+// One restructuring round: one thread per triangle walks up; the warp restructures the treelets its lanes own, one at a time.
+__global__ void __launch_bounds__(32 * TREELET_WARPS)
+    k_treelet(int n, const float* __restrict__ tri_aabb, const uint32_t* __restrict__ prim, int2* children, int* parent, float* node_aabb, int* sizes,
+              float* cost, int* height, int* as_leaf, const int* __restrict__ depth, int* flags, int max_depth)
+{
+    __shared__ Treelet sh[TREELET_WARPS];
+    Treelet&           t    = sh[threadIdx.x >> 5];
+    const int          k    = blockIdx.x * blockDim.x + threadIdx.x;
+    int                node = k < n ? __ldcg(parent + n - 1 + k) : -1;
+    bool               active = node >= 0;
+    while (__any_sync(0xFFFFFFFFu, active))
+    {
+        bool ready = false;
+        if (active)
+        {
+            ready  = atomicAdd(flags + node, 1) != 0; // first arrival: the sibling subtree is not finished yet
+            active = ready;
+            __threadfence();
+        }
+        __syncwarp();
+        for (unsigned todo = __ballot_sync(0xFFFFFFFFu, ready); todo; todo &= todo - 1)
+        {
+            const int root = __shfl_sync(0xFFFFFFFFu, node, __ffs(todo) - 1);
+            treelet_node(t, root, n, tri_aabb, prim, children, parent, node_aabb, sizes, cost, height, as_leaf, depth, max_depth);
+        }
+        if (ready)
+        {
+            node   = __ldcg(parent + node);
+            active = node >= 0;
+        }
+    }
+}
+
+// depth of every internal node (edges from the root)
+__global__ void k_node_depth(int n, const int* __restrict__ parent, int* __restrict__ depth)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n - 1) return;
+    int d = 0;
+    for (int cur = i; d < (1 << 20) && parent[cur] >= 0; cur = parent[cur]) d++;
+    depth[i] = d;
+}
+
 } // namespace
 
 int g_hr_bvh_quality = 1;
+int g_hr_bvh_treelet_rounds = 3;
+
+extern "C" HR_API int hr_internal_bvh_treelet_rounds(int rounds)
+{
+    const int prev = g_hr_bvh_treelet_rounds;
+    if (rounds >= 0) g_hr_bvh_treelet_rounds = rounds;
+    return prev;
+}
 
 namespace {
 
-// Builds children / ranges / node_aabb (and the depth-first primitive order in sc->d_vals) with PLOC.
+// Builds children / ranges / node_aabb (and the depth-first primitive order in sc->d_vals) with PLOC, then restructures its
+// treelets for g_hr_bvh_treelet_rounds rounds; *as_leaf is the per-node leaf choice for k_pack_nodes (null without rounds).
 // Returns HR_OK, a negative hr_status on a CUDA error, or 1 if the round cap is hit (caller falls back to the radix tree).
-int ploc_build(hr_scene* sc, cudaStream_t st)
+int ploc_build(hr_scene* sc, cudaStream_t st, const int** as_leaf)
 {
     hr_ctx*   ctx = sc->ctx;
     const int n   = (int)sc->n_tris;
@@ -417,7 +665,8 @@ int ploc_build(hr_scene* sc, cudaStream_t st)
     size_t scan_tmp = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (unsigned long long*)nullptr, (unsigned long long*)nullptr, n, st);
     const size_t o_c0 = 0, o_c1 = o_c0 + sizeof(Cluster) * n, o_nn = o_c1 + sizeof(Cluster) * n, o_fl = o_nn + ((sizeof(int) * n + 15) & ~size_t(15)),
-                 o_sc = o_fl + 8ull * n, o_cnt = o_sc + 8ull * n, o_tmp = o_cnt + 16, total = o_tmp + scan_tmp;
+                 o_sc = o_fl + 8ull * n, o_cnt = o_sc + 8ull * n, o_tmp = o_cnt + 16, o_tl = (o_tmp + scan_tmp + 15) & ~size_t(15),
+                 total = o_tl + 5ull * sizeof(int) * n;
     if (total > sc->ploc_bytes)
     {
         if (sc->d_ploc) cudaFree(sc->d_ploc);
@@ -453,6 +702,25 @@ int ploc_build(hr_scene* sc, cudaStream_t st)
         cur ^= 1;
     }
     if (node_base != 0) return 1;
+    *as_leaf = nullptr;
+    if (g_hr_bvh_treelet_rounds > 0)
+    {
+        // treelet scratch: SAH cost, height, leaf choice, depth and walk flags of every internal node
+        float* cost   = (float*)(base + o_tl);
+        int*   height = (int*)(base + o_tl) + n;
+        int*   leaf   = height + n;
+        int*   depth  = leaf + n;
+        int*   tflags = depth + n;
+        for (int r = 0; r < g_hr_bvh_treelet_rounds; r++)
+        {
+            HR_CUDA(ctx, cudaMemsetAsync(tflags, 0, sizeof(int) * (n - 1), st));
+            k_node_depth<<<(n - 1 + T - 1) / T, T, 0, st>>>(n, sc->d_parent, depth);
+            k_treelet<<<(n + 32 * TREELET_WARPS - 1) / (32 * TREELET_WARPS), 32 * TREELET_WARPS, 0, st>>>(
+                n, sc->d_tri_aabb, sc->d_vals_sorted, sc->d_children, sc->d_parent, sc->d_node_aabb, sizes, cost, height, leaf, depth, tflags, HR_BVH_MAX_DEPTH);
+            ctx->launches += 2;
+        }
+        *as_leaf = leaf;
+    }
     int* leaf_pos = reinterpret_cast<int*>(sc->d_keys); // the unsorted keys / values are dead after the radix sort
     k_ploc_offsets<<<(2 * n - 1 + T - 1) / T, T, 0, st>>>(n, sc->d_children, sc->d_parent, sizes, sc->d_vals_sorted, sc->d_ranges, leaf_pos, sc->d_vals);
     k_ploc_remap<<<(n - 1 + T - 1) / T, T, 0, st>>>(n, sc->d_children, leaf_pos);
@@ -489,21 +757,23 @@ int hr_bvh_build(hr_scene* sc, cudaStream_t st)
     {
         const int gi = (int)((n - 1 + T - 1) / T);
         bool      ploc = false;
+        const int* as_leaf = nullptr;
         if (g_hr_bvh_quality >= 1)
         {
-            const int rc = ploc_build(sc, st);
+            const int rc = ploc_build(sc, st, &as_leaf);
             if (rc < 0) return rc; // CUDA error, already recorded (rc > 0: round cap hit, fall back to the radix tree)
             ploc = rc == HR_OK;
         }
         if (ploc) prim_order = sc->d_vals;
         else
         {
+            as_leaf = nullptr;
             HR_CUDA(ctx, cudaMemsetAsync(sc->d_flags, 0, sizeof(int) * (n - 1), st));
             k_hierarchy<<<gi, T, 0, st>>>(sc->d_keys_sorted, (int)n, sc->d_children, sc->d_ranges, sc->d_parent);
             k_fit<<<gb, T, 0, st>>>(sc->d_tri_aabb, sc->d_vals_sorted, (int)n, sc->d_children, sc->d_parent, sc->d_node_aabb, sc->d_flags);
             ctx->launches += 2;
         }
-        k_pack_nodes<<<gi, T, 0, st>>>((int)n, sc->d_children, sc->d_ranges, sc->d_tri_aabb, prim_order, sc->d_node_aabb, sc->d_bounds_i, sc->d_nodes);
+        k_pack_nodes<<<gi, T, 0, st>>>((int)n, sc->d_children, sc->d_ranges, as_leaf, sc->d_tri_aabb, prim_order, sc->d_node_aabb, sc->d_bounds_i, sc->d_nodes);
         HR_CUDA(ctx, cudaMemsetAsync(sc->d_depth, 0, sizeof(int), st));
         k_depth<<<gb, T, 0, st>>>((int)n, sc->d_parent, sc->d_depth);
         sc->n_nodes = n - 1;

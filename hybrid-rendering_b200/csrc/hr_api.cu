@@ -453,6 +453,19 @@ int hr_scene_set_textures(hr_scene* sc, const hr_texture* textures, size_t n_tex
 int hr_scene_set_current(hr_ctx* ctx, hr_scene* scene) { if (!ctx) return HR_ERR_INVALID_ARG; ctx->scene = scene; return HR_OK; }
 int hr_scene_get_info(hr_scene* sc, hr_scene_info* out) { if (!sc || !out) return HR_ERR_INVALID_ARG; *out = sc->info; return HR_OK; }
 
+int hr_scene_download_bvh(hr_scene* sc, void* nodes, size_t nodes_bytes, void* tris, size_t tris_bytes)
+{
+    if (!sc) return HR_ERR_INVALID_ARG;
+    hr_ctx* ctx = sc->ctx;
+    HR_REQUIRE(ctx, !nodes || nodes_bytes == sc->n_nodes * 4 * sizeof(float4), HR_ERR_INVALID_ARG, "hr_scene_download_bvh: nodes_bytes must be n_nodes * 64");
+    HR_REQUIRE(ctx, !tris || tris_bytes == sc->n_tris * 3 * sizeof(float4), HR_ERR_INVALID_ARG, "hr_scene_download_bvh: tris_bytes must be n_triangles * 48");
+    HR_CUDA(ctx, cudaSetDevice(ctx->device));
+    HR_CUDA(ctx, cudaDeviceSynchronize());
+    if (nodes) HR_CUDA(ctx, cudaMemcpy(nodes, sc->d_nodes, nodes_bytes, cudaMemcpyDeviceToHost));
+    if (tris) HR_CUDA(ctx, cudaMemcpy(tris, sc->d_tris, tris_bytes, cudaMemcpyDeviceToHost));
+    return HR_OK;
+}
+
 int hr_trace_any(hr_ctx* ctx, const float* d_rays, size_t n, uint32_t* d_out, void* stream)
 {
     HR_REQUIRE(ctx, ctx && ctx->scene, HR_ERR_NOT_READY, "hr_trace_any: no current scene");

@@ -378,6 +378,9 @@ void launch_drain_ray_counters(unsigned long long* ctr, unsigned long long* d_ou
 void launch_checksum(const void* base, int texel_bytes, size_t texel0, size_t texel1, unsigned long long* d_out, cudaStream_t st);
 int hr_launch_build_mips(hr_ctx* ctx, GBufSlot& s, int W, int H, cudaStream_t st);
 int hr_bvh_build(hr_scene* sc, cudaStream_t st);
+// Test hook, exported but not part of hr_api.h: treelet restructuring rounds of the PLOC build (default 3; 0 = plain PLOC, the
+// baseline tests compare the restructured tree against).  rounds < 0 only queries.  Returns the previous value.
+extern "C" HR_API int hr_internal_bvh_treelet_rounds(int rounds);
 BvhDev hr_bvh_view(const hr_scene* sc);
 
 // Function attributes (opt-in shared memory sizes) are per device: launchers keep one flag per device, not per process, so

@@ -126,7 +126,7 @@ HR_FMT = {1: ("<u4", 1), 2: ("<f2", 1), 3: ("<f2", 2), 4: ("<f2", 4), 5: ("u1", 
 # every symbol include/hr_api.h declares (checked by tests/test_abi.py)
 ABI_SYMBOLS = [
     "hr_init", "hr_shutdown", "hr_last_error", "hr_version", "hr_bluenoise_set", "hr_scene_build", "hr_scene_destroy", "hr_scene_set_current",
-    "hr_scene_get_info", "hr_scene_rebuild", "hr_trace_any", "hr_trace_closest", "hr_gbuffer_create", "hr_gbuffer_upload",
+    "hr_scene_get_info", "hr_scene_rebuild", "hr_scene_download_bvh", "hr_trace_any", "hr_trace_closest", "hr_gbuffer_create", "hr_gbuffer_upload",
     "hr_gbuffer_stage_upload", "hr_gbuffer_commit_staged", "hr_pass_download_async", "hr_pass_download_rows_async",
     "hr_gbuffer_copy_from_device", "hr_gbuffer_bind_device", "hr_gbuffer_download", "hr_shadows_default_params", "hr_shadows_create",
     "hr_shadows_render", "hr_ao_default_params", "hr_ao_create", "hr_ao_render", "hr_pass_output", "hr_pass_download", "hr_pass_reset_history",
@@ -446,6 +446,15 @@ class Context:
         info = hr_scene_info()
         self.check(self.lib.hr_scene_get_info(scene, C.byref(info)), "hr_scene_get_info")
         return info
+
+    def download_bvh(self, scene):
+        """hr_scene_download_bvh: (nodes float32 (n_nodes, 4, 4), tris float32 (n_triangles, 3, 4)) in the traversal layout"""
+        info = self.scene_info(scene)
+        nodes = np.empty((info.n_nodes, 4, 4), np.float32)
+        tris = np.empty((info.n_triangles, 3, 4), np.float32)
+        self.check(self.lib.hr_scene_download_bvh(scene, _ptr(nodes), C.c_size_t(nodes.nbytes), _ptr(tris), C.c_size_t(tris.nbytes)),
+                   "hr_scene_download_bvh")
+        return nodes, tris
 
     def gbuffer_create(self, W, H):
         self.check(self.lib.hr_gbuffer_create(self.h, W, H), "hr_gbuffer_create")

@@ -142,8 +142,8 @@ typedef struct hr_instance {
 } hr_instance;
 
 /* Builds the device BVH over all instances' world-space triangles: 63-bit Morton codes + radix sort, then PLOC
- * agglomerative clustering (default) or the Karras radix tree + bottom-up fit (hr_debug_set key 3), collapsed into
- * <= 4-triangle leaves and packed into 64-byte two-child nodes.  Host pointers in; synchronises the context's build
+ * agglomerative clustering with treelet restructuring for the surface-area cost (default) or the Karras radix tree + bottom-up
+ * fit (hr_debug_set key 3), collapsed into <= 2-triangle leaves and packed into 64-byte two-child nodes.  Host pointers in; synchronises the context's build
  * stream before returning.  Fails with HR_ERR_UNSUPPORTED when the tree is deeper than the traversal stack (64).  Every
  * built scene gets a new process-wide serial number; a DDGI pass re-initialises its probe grid when it next renders a scene
  * with another serial, even one allocated at a destroyed scene's address. */
@@ -165,6 +165,11 @@ typedef struct hr_scene_info {
 HR_API int hr_scene_get_info(hr_scene* scene, hr_scene_info* out);
 /* Re-run only the device build (the reference rebuilds its TLAS every frame, src/main.cpp:74). */
 HR_API int hr_scene_rebuild(hr_scene* scene, void* stream);
+/* Read-only copy of the built tree to host memory, for measuring its quality: the traversal layout of bvh_build.cu, n_nodes
+ * nodes of 4 float4 (both child boxes, then the child links; child < 0 is a leaf ~((first << 3) | (count - 1))) and n_triangles
+ * triangles of 3 float4 (v0 with the primitive index's bits in w, e1, e2) in leaf order.  nodes_bytes must be n_nodes * 64 and
+ * tris_bytes n_triangles * 48; a NULL destination is skipped.  Synchronises the device. */
+HR_API int hr_scene_download_bvh(hr_scene* scene, void* nodes, size_t nodes_bytes, void* tris, size_t tris_bytes);
 
 /* Material textures (Material::load + the bindless s_Textures array, extras/ray_traced_scene.cpp:345-420, scene_descriptor_set.glsl:84-93,180-218).
  * textures: 8-bit images, 1, 2 or 4 channels (what Image::create_from_file produces: RGB files arrive as RGBA), host pointers, copied;
