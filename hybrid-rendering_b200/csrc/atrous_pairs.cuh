@@ -1,5 +1,5 @@
-// atrous_pairs.cuh — the pixel-pair a-trous tile kernels of the shadows (svgf_atrous_v3.cu, K4+K5) and reflections
-// (svgf_refl_atrous_v2.cu, K15+K16) denoisers.
+// atrous_pairs.cuh — the pixel-pair a-trous tile kernels of the shadows (svgf_atrous.cu, K4+K5) and reflections
+// (svgf_refl_atrous.cu, K15+K16) denoisers.
 //
 // The scalar a-trous kernels are instruction-issue bound: ~23 FP32 instructions per tap.  Here every thread filters TWO
 // horizontally adjacent pixels and keeps each per-pixel quantity of the pair in one 64-bit register pair (gf::ffma2 / fmul2 /
@@ -24,8 +24,8 @@
 #include "glsl_fast.cuh"
 #include "hr_internal.h"
 
-// File-local in each including file, like the kernels.  The dynamic shared-memory array stays a file-local symbol declared
-// after the TMA kernel's 128-byte-aligned one, and ptxas keeps the reflections kernels' dynamic window at the 128-byte offset.
+// File-local in each including file, like the kernels.  ptxas starts the dynamic shared memory of every kernel of a file at the
+// largest alignment of the file's dynamic shared-memory arrays: 128 bytes in svgf_refl_atrous.cu (the TMA kernel's boxes).
 namespace {
 
 constexpr int PAIR_TILE_W = 64, PAIR_TILE_H = 16;

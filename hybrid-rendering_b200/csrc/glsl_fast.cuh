@@ -19,6 +19,13 @@ __device__ __forceinline__ float4 h4_to_f4(uint2 w)
     const float2 a = h2_to_f2(w.x), b = h2_to_f2(w.y);
     return make_float4(a.x, a.y, b.x, b.y);
 }
+__device__ __forceinline__ uint2 pack_h4(float a, float b, float c, float d) { return make_uint2(f2_to_h2(a, b), f2_to_h2(c, d)); }
+
+// common.glsl:143
+__device__ __forceinline__ float luminance(float r, float g, float b) { return fmaxf(r * 0.299f + g * 0.587f + b * 0.114f, 0.0001f); }
+
+// textureLod NEAREST + CLAMP_TO_EDGE: texel = clamp(floor(uv * size), 0, size-1)
+__device__ __forceinline__ int nearest(float uv, int size) { return min(max((int)floorf(uv * (float)size), 0), size - 1); }
 
 // Pixel-pair arithmetic of the a-trous kernels: one correctly rounded FFMA / FMUL / FADD per lane of the pair, never
 // contracted or reassociated, so both pixels get exactly what the scalar kernel computes.

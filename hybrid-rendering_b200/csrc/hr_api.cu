@@ -11,9 +11,6 @@
 
 static std::string g_last_error;
 static std::mutex  g_err_mutex;
-extern int         g_hr_atrous_impl;
-extern int         g_hr_bvh_quality;
-extern int         g_hr_refl_atrous_impl;
 
 void hr_set_error(hr_ctx* ctx, const char* fmt, ...)
 {

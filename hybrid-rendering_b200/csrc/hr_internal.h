@@ -287,7 +287,7 @@ struct hr_pass {
     std::vector<void*> allocs;
 };
 
-// rt_shade.cu / ddgi_update.cu / svgf_reflections.cu
+// rt_shade.cu / ddgi_update.cu
 void launch_ddgi_ray_trace(const hr_scene* sc, const hr_ddgi_uniforms& d, const void* irr_prev, const void* depth_prev, const hr_light& light, const float* rot16,
                            uint32_t num_frames, uint32_t infinite_bounces, float gi_intensity, const float* sky3, int probe0, int probe1, void* radiance,
                            void* dirdepth, unsigned long long* ray_ctr, cudaStream_t st);
@@ -299,14 +299,6 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
                                   float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
                                   const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
                                   int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st); // chunk_stride > 1: only the 8-row chunks c = chunk_first + i * chunk_stride (rows are ignored)
-void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const void* input, const HistPeers& hist, const FrameConsts& fc, float alpha,
-                                 float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
-int  launch_reflections_atrous(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
-                               float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st);
-// svgf_refl_atrous_v2.cu: the pixel-pair kernels of launch_reflections_atrous; false when they do not support the call
-bool launch_reflections_atrous_v2(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
-                                  float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st);
-void launch_upsample_vec4(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, void* out, int row0, int row1, cudaStream_t st);
 
 // ---- row-band sharding (shard.cu) ---------------------------------------------------------------------
 // An image whose rows are owned band-wise by the ranks.  The band partition is defined on the PASS height `H`
@@ -406,16 +398,29 @@ void launch_ray_trace_shared(int kind, const GBufLevelDev& g, const BvhDev& bvh,
 void launch_trace_any(const BvhDev& bvh, const float* rays, size_t n, uint32_t* out, cudaStream_t st);
 void launch_trace_closest(const BvhDev& bvh, const float* rays, size_t n, float* out_t, uint32_t* out_prim, float* out_uv, cudaStream_t st);
 
+// ---- SVGF denoise stages: one launcher per stage holds the whole kernel selection ----------------------------------------
 // svgf_temporal.cu: K3 (PASS_SHADOWS: out_img RG16F, out_aux moments RGBA16F) or K9 (PASS_AO: out_img R16F, out_aux history length
 // R16F; moments_alpha unused), the visibility from `mask` at spp 1 or from `count` at spp > 1
 void launch_temporal(int kind, const GBufLevelDev& cur, const GBufLevelDev& prev, const uint32_t* mask, const uint8_t* count, int spp, const HistPeers& hist,
                      const FrameConsts& fc, float alpha, float moments_alpha, void* out_img, void* out_aux, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
+// svgf_temporal.cu: K14
+void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const void* input, const HistPeers& hist, const FrameConsts& fc, float alpha,
+                                 float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st);
+// svgf_atrous.cu: K5
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st);
-// svgf_atrous_v3.cu: the pixel-pair kernels of launch_shadows_atrous; false when they do not support the call
-bool launch_shadows_atrous_v3(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n, float sigma_z,
-                              float power, uint32_t* out, int row0, int row1, cudaStream_t st);
+// svgf_refl_atrous.cu: K16; -1 when radius != 1 or step is not a power of two <= 16
+int  launch_reflections_atrous(const GBufLevelDev& g, const void* in, const uint8_t* tile_flags, int radius, int step, float phi_color, float phi_normal,
+                               float sigma_depth, int approximate_with_ddgi, void* out, int row0, int row1, unsigned int* counters, cudaStream_t st);
+// svgf_misc.cu: K6 / K11 (scalar) and K17 (RGBA16F) upsample, K10 AO blur
 void launch_upsample_scalar(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, int in_channels, float sky_value, float power,
                             __half* out, int row0, int row1, cudaStream_t st);
+void launch_upsample_vec4(const GBufLevelDev& g0, const GBufLevelDev& gm, const void* in, void* out, int row0, int row1, cudaStream_t st);
 void launch_ao_blur(const GBufLevelDev& g, const __half* in, const uint8_t* tile_flags, const float* zbp, int dirx, int diry, int radius, __half* out,
                     int row0, int row1, cudaStream_t st);
+
+// hr_debug_set keys (include/hr_api.h), process-wide.  Whatever the key, the pixel-pair kernels fall back to the scalar ones for odd
+// widths, phi_normal != 32 and bands that do not start on a tile row.
+extern int g_hr_atrous_impl;      // key 1 (svgf_atrous.cu): 3 = pixel pairs (default), 1 = scalar tiled kernel, 0 = naive kernel
+extern int g_hr_refl_atrous_impl; // key 6 (svgf_refl_atrous.cu): 3 = 2 + TMA-staged step 1 (default), 2 = pixel pairs, 0 = scalar kernel
+extern int g_hr_bvh_quality;      // key 3 (bvh_build.cu): 1 = PLOC (default), 0 = Karras radix tree

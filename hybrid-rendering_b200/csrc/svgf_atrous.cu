@@ -3,21 +3,26 @@
 //   K5  shadows/shadows_denoise_atrous.comp:94-174 + edge_stopping.glsl:10-62
 // Algorithmic traffic per pixel and iteration (SURVEY.md §8d): RG16F in 4 + GB2 8 + GB3 8 read, RG16F 4 written = 24 B.
 //
-// Tiled kernel: one CTA filters a 64x16 output tile.  The tile plus a halo of `step` texels of
-//   * the input image (visibility, variance) as float2
-//   * the decoded G-buffer normal + linear z as float4 (oct decode done ONCE per staged texel, not once per tap)
-// is staged in shared memory with coalesced 8-byte/4-byte global loads (out-of-image texels are staged as zeros =
-// texelFetch robust-access semantics); the 3x3 taps at stride `step` then come from shared memory.
-// A CTA whose 16 reference tiles are all on the shadow list writes zeros and exits without loading anything.
-#include "glsl_fast.cuh"
-#include "hr_internal.h"
+// Three kernel forms, chosen by launch_shadows_atrous:
+//   k_atrous_v3 / k_atrous_v3s  pixel pairs (atrous_pairs.cuh), the default.  Six staged planes: nx, ny, nz, z*log2e/sigma,
+//                               visibility, variance.  The visibility is the one colour channel and also the luminance the
+//                               colour weight compares.
+//   k_atrous_tiled              the scalar tiled kernel: odd widths, phi_normal != 32, and the reference of the pixel pairs.
+//                               One CTA filters a 64x16 output tile.  The tile plus a halo of `step` texels of
+//                                 * the input image (visibility, variance) as float2
+//                                 * the decoded G-buffer normal + linear z as float4 (oct decode done ONCE per staged texel)
+//                               is staged in shared memory with coalesced 8-byte/4-byte global loads (out-of-image texels are
+//                               staged as zeros = texelFetch robust-access semantics); the 3x3 taps at stride `step` then come
+//                               from shared memory.  A CTA whose 16 reference tiles are all on the shadow list writes zeros and
+//                               exits without loading anything.
+//   k_atrous_naive              global memory only: radius != 1 and steps >= 16.
+#include "atrous_pairs.cuh"
 
 namespace {
 
 using namespace gf;
 
-constexpr int TILE_W = 64, TILE_H = 16, MAX_STEP = 8;
-constexpr int REG_W_MAX = TILE_W + 2 * MAX_STEP, REG_H_MAX = TILE_H + 2 * MAX_STEP;
+constexpr int TILE_W = 64, TILE_H = 16;
 
 struct AtrousParams {
     int   W, H, step, radius;
@@ -172,7 +177,6 @@ __global__ void __launch_bounds__(256) k_atrous_tiled(GBufLevelDev g, const uint
     }
 }
 
-
 template <int STEP>
 void launch_tiled(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, const AtrousParams& P, uint32_t* out, cudaStream_t st)
 {
@@ -184,24 +188,118 @@ void launch_tiled(const GBufLevelDev& g, const uint32_t* in, const uint8_t* tf, 
     k_atrous_tiled<STEP><<<grid, 256, smem, st>>>(g, in, tf, P, out);
 }
 
+// ---- pixel-pair kernels ------------------------------------------------------------------------------------------
+struct V3Params {
+    int   W, H;
+    float c_sigma;   // log2(e) / sigma_depth
+    float c_phi0;    // -log2(e) / phi_visibility
+    float power;
+    int   row0, row1;
+};
+
+struct ShadowsPass {
+    using In = uint32_t; using Out = uint32_t; using Params = V3Params;
+    static constexpr int  NPL = 6, NC = 1;
+    static constexpr bool COPY_EMPTY_CTA = false; // a CTA without a flagged tile stages nothing and writes zeros
+
+    // Stage the texel pair (px, px+1) of row py (px even) at region index ri (even): decoded normal, scaled linear depth, visibility,
+    // variance; zeros outside the image.
+    static __device__ __forceinline__ void stage(const GBufLevelDev& g, const uint32_t* __restrict__ in, float c_sigma, int px, int py, int W, int H, int ri, float* s, int PL)
+    {
+        float2 nx = make_float2(0.0f, 0.0f), ny = nx, nz = nx, zs = nx, vi = nx, va = nx;
+        if (px >= 0 && py >= 0 && px < W && py < H)
+        {
+            const size_t pi = (size_t)py * W + px;
+            const uint4  a  = __ldg(reinterpret_cast<const uint4*>(g.gb2 + pi)); // two RGBA16F texels: .x / .z hold the oct normals
+            const uint4  b  = __ldg(reinterpret_cast<const uint4*>(g.gb3 + pi)); // .y / .w hold (mesh id, linear z)
+            const uint2  c  = __ldg(reinterpret_cast<const uint2*>(in + pi));    // two RG16F texels (visibility, variance)
+            const float2 e0 = h2_to_f2(a.x), e1 = h2_to_f2(a.z);
+            const float3 n0 = octohedral_to_direction(e0.x, e0.y), n1 = octohedral_to_direction(e1.x, e1.y);
+            const float2 i0 = h2_to_f2(c.x), i1 = h2_to_f2(c.y);
+            nx = make_float2(n0.x, n1.x); ny = make_float2(n0.y, n1.y); nz = make_float2(n0.z, n1.z);
+            zs = make_float2(h2_to_f2(b.y).y * c_sigma, h2_to_f2(b.w).y * c_sigma);
+            vi = make_float2(i0.x, i1.x); va = make_float2(i0.y, i1.y);
+        }
+        float* p = s + ri;
+        *reinterpret_cast<float2*>(p) = nx; p += PL;
+        *reinterpret_cast<float2*>(p) = ny; p += PL;
+        *reinterpret_cast<float2*>(p) = nz; p += PL;
+        *reinterpret_cast<float2*>(p) = zs; p += PL;
+        *reinterpret_cast<float2*>(p) = vi; p += PL;
+        *reinterpret_cast<float2*>(p) = va;
+    }
+
+    static __device__ __forceinline__ float2 side_var(const uint32_t* __restrict__ in, size_t pi)
+    {
+        const uint2 w = __ldg(reinterpret_cast<const uint2*>(in + pi));
+        return make_float2(h2_to_f2(w.x).y, h2_to_f2(w.y).y);
+    }
+
+    template <bool ALIGNED_X>
+    static __device__ __forceinline__ void filter_store(const GBufLevelDev&, const V3Params& P, const PairTaps& t, uint32_t* __restrict__ out, size_t idx, bool has1, bool flagged)
+    {
+        if (!flagged)
+        {
+            out[idx] = 0u;
+            if (has1) out[idx + 1] = 0u;
+            return;
+        }
+        const PairSum<1> f  = filter_pair<1, 4, ALIGNED_X>(t, P.c_phi0); // luminance = visibility
+        float2           o0 = f.c[0];
+        if (P.power != 0.0f) { o0.x = pow_pos(o0.x, P.power); o0.y = pow_pos(o0.y, P.power); }
+        // sky pixels (linear z < 0) pass the input through
+        const float2   zs = ld_pair(t.s + 3 * t.PL, t.ci, true), vi = ld_pair(t.s + 4 * t.PL, t.ci, true), va = ld_pair(t.s + 5 * t.PL, t.ci, true);
+        const uint32_t r0 = zs.x < 0.0f ? f2_to_h2(vi.x, va.x) : f2_to_h2(o0.x, f.v.x);
+        const uint32_t r1 = zs.y < 0.0f ? f2_to_h2(vi.y, va.y) : f2_to_h2(o0.y, f.v.y);
+        if (has1) *reinterpret_cast<uint2*>(out + idx) = make_uint2(r0, r1); // idx even (W even is required by the launcher)
+        else out[idx] = r0;
+    }
+};
+
+template <int STEP>
+__global__ void __launch_bounds__(256) k_atrous_v3(GBufLevelDev g, const uint32_t* __restrict__ in, const uint8_t* __restrict__ tile_flags, V3Params P,
+                                                    uint32_t* __restrict__ out)
+{
+    atrous_dense<ShadowsPass, STEP>(g, in, tile_flags, P, out);
+}
+
+template <int STEP>
+__global__ void __launch_bounds__(256) k_atrous_v3s(GBufLevelDev g, const uint32_t* __restrict__ in, const uint8_t* __restrict__ tile_flags, V3Params P,
+                                                     uint32_t* __restrict__ out)
+{
+    atrous_interleaved<ShadowsPass, STEP>(g, in, tile_flags, P, out);
+}
+
+template <int STEP>
+using Dense = DenseTile<STEP, ShadowsPass::NPL>;
+template <int STEP>
+using Interleaved = InterleavedTile<STEP, ShadowsPass::NPL>;
+
 } // namespace
 
-// 0 = naive, 1 = tiled scalar kernel.  hr_debug_set key 1.  (A sliding-register-window "chain" variant, which traded
-// occupancy for shared-memory traffic, has been removed.)
-// 3 = pixel-pair kernel (svgf_atrous_v3.cu, default); it falls back to the
-// scalar tiled kernel for odd widths / phi_normal != 32.
 int g_hr_atrous_impl = 3;
 
 void launch_shadows_atrous(const GBufLevelDev& g, const __half2* in, const uint8_t* tile_flags, int radius, int step, float phi_vis, float phi_n,
                            float sigma_z, float power, __half2* out, int row0, int row1, cudaStream_t st)
 {
     if (row1 <= row0) return;
-    AtrousParams P { g.W, g.H, step, radius, phi_vis, phi_n, sigma_z, power, row0, row1 };
     const uint32_t* i32 = reinterpret_cast<const uint32_t*>(in);
     uint32_t*       o32 = reinterpret_cast<uint32_t*>(out);
-    const bool tiled_ok = g_hr_atrous_impl != 0 && radius == 1 && (step == 1 || step == 2 || step == 4 || step == 8);
-    if (g_hr_atrous_impl == 3 && launch_shadows_atrous_v3(g, i32, tile_flags, radius, step, phi_vis, phi_n, sigma_z, power, o32, row0, row1, st)) return;
-    if (tiled_ok)
+    const bool      tiled_step = radius == 1 && (step == 1 || step == 2 || step == 4 || step == 8);
+    if (g_hr_atrous_impl == 3 && tiled_step && phi_n == 32.0f && !(g.W & 1) && row0 % 8 == 0)
+    { // pixel pairs
+        V3Params P { g.W, g.H, 1.44269504f / sigma_z, -1.44269504f / phi_vis, power, row0, row1 };
+        switch (step)
+        {
+            case 1: launch_tiles<Dense<1>>(k_atrous_v3<1>, g, i32, tile_flags, P, o32, st); break;
+            case 2: launch_tiles<Dense<2>>(k_atrous_v3<2>, g, i32, tile_flags, P, o32, st); break;
+            case 4: launch_tiles<Dense<4>>(k_atrous_v3<4>, g, i32, tile_flags, P, o32, st); break;
+            default: launch_tiles<Interleaved<8>>(k_atrous_v3s<8>, g, i32, tile_flags, P, o32, st); break; // DESIGN.md §8
+        }
+        return;
+    }
+    AtrousParams P { g.W, g.H, step, radius, phi_vis, phi_n, sigma_z, power, row0, row1 };
+    if (g_hr_atrous_impl != 0 && tiled_step)
     {
         switch (step)
         {

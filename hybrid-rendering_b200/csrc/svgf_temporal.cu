@@ -1,11 +1,12 @@
-// svgf_temporal.cu — temporal reprojection + accumulation for the bit-mask effects.
+// svgf_temporal.cu — temporal reprojection + accumulation of the shadows, AO and reflections chains.
 //   K3  shadows/shadows_denoise_reprojection.comp:196-293  (+ reprojection.glsl:115-328, REPROJECTION_MOMENTS)
 //   K9  ao/ao_denoise_reprojection.comp:191-260            (history length in its own R16F image)
+//   K14 reflections/reflections_denoise_reprojection.comp:174-289 (+ reprojection.glsl:78-111,115-328 REPROJECTION_REFLECTIONS)
 // K2/K8 (reset_args) and the tile *lists* are replaced by a per-8x8-tile flag byte (1 = denoise list): the lists' order
 // is non-deterministic in the reference (atomicAdd) and only membership matters.
 //
 // One CTA = 32x8 pixels (4 reference tiles), one warp per pixel row => every G-buffer / history row access is a
-// contiguous 32-pixel span.  The 17x17 box mean of the packed ray mask is computed from 24 64-bit row bitmaps held in
+// contiguous 32-pixel span.  K3/K9: the 17x17 box mean of the packed ray mask is computed from 24 64-bit row bitmaps held in
 // shared memory: count = sum_rows popcll(row & window) — exact (integers <= 289), like the reference's float sums.
 // With spp > 1 the same kernel reads the 8-bit count image instead (k_temporal's COUNT).
 #include "glsl_fast.cuh"
@@ -31,6 +32,50 @@ __device__ __forceinline__ HistTap fetch_prev(const GBufLevelDev& p, int x, int 
     return t;
 }
 
+// ---- history fetches through the owner table (HistPeers, hr_internal.h) ----
+// Rows owned by this GPU use the read-only path; rows owned by a peer are read over NVLink with L1 bypassed (the mapping
+// is rewritten by the peer every frame).  A warp's 32 pixels share their row in the static case, so the branch is uniform.
+__device__ __forceinline__ int owner_of(const HistPeers& hp, int row)
+{
+    int o = 0;
+#pragma unroll
+    for (int r = 0; r < HR_MAX_RANKS - 1; r++) o += (r < hp.world - 1 && row >= hp.band_end[r]) ? 1 : 0;
+    return o;
+}
+// The rank that owns a history row: `uniform` when one rank owns every row a pixel reads (k_refl_temporal looks it up once per
+// pixel), otherwise owner_of per load.
+struct HistOwner { int o; bool uniform; };
+
+// element `index` of a history image (hp.img or hp.aux) in row `row`, read as T; a 16-bit T is returned zero-extended to 32 bits
+template <bool PEER, class T>
+__device__ __forceinline__ std::conditional_t<(sizeof(T) < 4), uint32_t, T> hist_ld(const void* const* tab, const HistPeers& hp, const HistOwner& ho, int row,
+                                                                                      size_t index)
+{
+    if (hp.no_history) return {};
+    if (!PEER) return __ldg(reinterpret_cast<const T*>(tab[0]) + index);
+    const int o = ho.uniform ? ho.o : owner_of(hp, row);
+    const T*  p = reinterpret_cast<const T*>(tab[o]) + index;
+    return o == hp.self ? __ldg(p) : __ldcg(p);
+}
+
+// Tile classification of a 32x8 CTA: 4 tiles of 8 columns.  Each warp ORs the tiles its row flags into the shared word s_flags
+// (zeroed by the kernel before its first barrier), then one flag byte per tile is stored.  A macro, not a function: an inlined
+// call renumbers the registers of k_temporal's count forms, and both kernels keep the generated code they were tuned with.
+#define STORE_TILE_FLAGS(flag, s_flags, lx, x0, y0, W, H, row1, tile_flags)                                                         \
+    do {                                                                                                                            \
+        const uint32_t _b = __ballot_sync(0xFFFFFFFFu, (flag));                                                                     \
+        if ((lx) == 0 && _b)                                                                                                        \
+            atomicOr(&(s_flags), ((_b & 0xFFu) ? 1u : 0u) | ((_b & 0xFF00u) ? 2u : 0u) | ((_b & 0xFF0000u) ? 4u : 0u) |             \
+                                     ((_b & 0xFF000000u) ? 8u : 0u));                                                               \
+        __syncthreads();                                                                                                            \
+        if (threadIdx.x < 4)                                                                                                        \
+        {                                                                                                                           \
+            const int _tx = ((x0) >> 3) + threadIdx.x, _ty = (y0) >> 3, _TW = ((W) + 7) >> 3;                                       \
+            if (_tx < _TW && (y0) < (H) && (y0) < (row1)) (tile_flags)[(size_t)_ty * _TW + _tx] = ((s_flags) >> threadIdx.x) & 1u; \
+        }                                                                                                                           \
+    } while (0)
+
+// ---- K3 / K9 ----
 struct TapRaw { uint32_t e, g3; float depth; };
 
 __device__ __forceinline__ TapRaw fetch_prev_raw(const GBufLevelDev& p, size_t i)
@@ -48,41 +93,12 @@ __device__ __forceinline__ HistTap decode_tap(const TapRaw& r)
     return HistTap { e.x, e.y, h2_to_f2(r.g3).x, r.depth };
 }
 
-// ---- history fetches through the owner table (HistPeers, hr_internal.h) ----
-// Rows owned by this GPU use the read-only path; rows owned by a peer are read over NVLink with L1 bypassed (the mapping
-// is rewritten by the peer every frame).  A warp's 32 pixels share their row in the static case, so the branch is uniform.
-__device__ __forceinline__ int owner_of(const HistPeers& hp, int row)
-{
-    int o = 0;
-#pragma unroll
-    for (int r = 0; r < HR_MAX_RANKS - 1; r++) o += (r < hp.world - 1 && row >= hp.band_end[r]) ? 1 : 0;
-    return o;
-}
-template <bool PEER>
-__device__ __forceinline__ uint32_t hist_ld32(const void* const* tab, const HistPeers& hp, int row, size_t word_index)
-{
-    if (hp.no_history) return 0u;
-    if (!PEER) return __ldg(reinterpret_cast<const uint32_t*>(tab[0]) + word_index);
-    const int       o = owner_of(hp, row);
-    const uint32_t* p = reinterpret_cast<const uint32_t*>(tab[o]) + word_index;
-    return o == hp.self ? __ldg(p) : __ldcg(p);
-}
-template <bool PEER>
-__device__ __forceinline__ uint32_t hist_ld16(const void* const* tab, const HistPeers& hp, int row, size_t half_index)
-{
-    if (hp.no_history) return 0u;
-    if (!PEER) return __ldg(reinterpret_cast<const unsigned short*>(tab[0]) + half_index);
-    const int             o = owner_of(hp, row);
-    const unsigned short* p = reinterpret_cast<const unsigned short*>(tab[o]) + half_index;
-    return o == hp.self ? __ldg(p) : __ldcg(p);
-}
-
 // visibility input: the 1-spp ray mask (one word per 8x4 pixel block), or the spp > 1 count image (unoccluded rays per pixel)
 template <bool COUNT> struct VisIn { const uint32_t* mask; };
 template <> struct VisIn<true> { const uint8_t* count; int spp; };
 
 // MODE 0: shadows (history RG16F .r, moments RGBA16F (m1,m2,N,0)); MODE 1: AO (history R16F, length R16F).
-// PEER: linked ranks read a history texel from the rank that owns its row (hist_ld32 / hist_ld16).
+// PEER: linked ranks read a history texel from the rank that owns its row (hist_ld).
 // COUNT (spp > 1, SURVEY.md §8d; not in the reference): the 17x17 box mean is the sum of an 8-bit count tile (separable:
 // 17-wide row sums, then 17 rows) divided by 289 * spp, the pixel's visibility is count / spp.
 template <int MODE, bool PEER, bool COUNT>
@@ -186,14 +202,15 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
             bool  valid = false;
             if (in_frame)
             {
+                const HistOwner per_load { 0, false }; // the owner of every history load is looked up for its row
                 // all history-side loads of the common path (<= 4 bilinear taps + history length) are issued back to back,
                 // before any of the validity arithmetic, so they share one HBM round trip
                 const float fx = hfx - floorf(hfx), fy = hfy - floorf(hfy);
                 const float w4[4] = { (1 - fx) * (1 - fy), fx * (1 - fy), (1 - fx) * fy, fx * fy };
                 {
                     const size_t hi = (size_t)hcy * W + hcx;
-                    if (MODE == 0) hist_len = h2_to_f2(hist_ld32<PEER>(hp.aux, hp, hcy, 2 * hi + 1)).x;
-                    else hist_len = __half2float(__ushort_as_half((unsigned short)hist_ld16<PEER>(hp.aux, hp, hcy, hi)));
+                    if (MODE == 0) hist_len = h2_to_f2(hist_ld<PEER, uint32_t>(hp.aux, hp, per_load, hcy, 2 * hi + 1)).x;
+                    else hist_len = __half2float(__ushort_as_half(hist_ld<PEER, unsigned short>(hp.aux, hp, per_load, hcy, hi)));
                 }
                 TapRaw   tr[4];
                 uint32_t hraw[4], mraw[4];
@@ -213,10 +230,10 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
                         tr[s] = fetch_prev_raw(prev, pi);
                         if (MODE == 0)
                         {
-                            hraw[s] = hist_ld32<PEER>(hp.img, hp, py, pi);
-                            mraw[s] = hist_ld32<PEER>(hp.aux, hp, py, 2 * pi);
+                            hraw[s] = hist_ld<PEER, uint32_t>(hp.img, hp, per_load, py, pi);
+                            mraw[s] = hist_ld<PEER, uint32_t>(hp.aux, hp, per_load, py, 2 * pi);
                         }
-                        else hraw[s] = hist_ld16<PEER>(hp.img, hp, py, pi);
+                        else hraw[s] = hist_ld<PEER, unsigned short>(hp.img, hp, per_load, py, pi);
                     }
                 }
                 const float3 cn   = rn_octohedral_to_direction(g2.x, g2.y);
@@ -258,12 +275,12 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
                                     const size_t pi = (size_t)py * W + px;
                                     if (MODE == 0)
                                     {
-                                        hcol += h2_to_f2(hist_ld32<PEER>(hp.img, hp, py, pi)).x;
-                                        const float2 mm = h2_to_f2(hist_ld32<PEER>(hp.aux, hp, py, 2 * pi));
+                                        hcol += h2_to_f2(hist_ld<PEER, uint32_t>(hp.img, hp, per_load, py, pi)).x;
+                                        const float2 mm = h2_to_f2(hist_ld<PEER, uint32_t>(hp.aux, hp, per_load, py, 2 * pi));
                                         hm0 += mm.x;
                                         hm1 += mm.y;
                                     }
-                                    else hcol += __half2float(__ushort_as_half((unsigned short)hist_ld16<PEER>(hp.img, hp, py, pi)));
+                                    else hcol += __half2float(__ushort_as_half(hist_ld<PEER, unsigned short>(hp.img, hp, per_load, py, pi)));
                                 }
                                 cntv += 1.0f;
                             }
@@ -314,19 +331,224 @@ __global__ void __launch_bounds__(256, 4) k_temporal(GBufLevelDev cur, GBufLevel
             flag = o0 < 1.0f;
         }
     }
-    // tile classification: 4 tiles of 8 columns per CTA
-    const uint32_t b = __ballot_sync(0xFFFFFFFFu, flag);
-    if (lx == 0 && b)
+    STORE_TILE_FLAGS(flag, s_flags, lx, x0, y0, W, H, row1, tile_flags);
+}
+
+// ---- K14 ----
+struct ReflTemporalParams { float alpha, moments_alpha; int approximate_with_ddgi; int row0, row1; int rot; }; // rot: the last `rot` tile rows are scheduled first
+
+// All history taps of a pixel lie in rows hcy-1 .. hcy+1: the owner is looked up once per pixel (two owner_of calls) and only
+// pixels whose taps straddle a band border fall back to a lookup per load.
+template <bool PEER>
+__device__ __forceinline__ HistOwner owner_cache(const HistPeers& hp, int row_lo, int row_hi)
+{
+    HistOwner c { 0, true };
+    if (PEER) { c.o = owner_of(hp, row_lo); c.uniform = c.o == owner_of(hp, row_hi); }
+    return c;
+}
+
+// CTA = 32x8 pixels.  17x17 mean / std-dev of the current ray-trace colour (neighborhood_standard_deviation :133-157; the
+// reference does 289 fetches per pixel): separable, each direction as a SLIDING window — stage the 48x24 rgb region; 144 threads
+// each walk half a staged row of one channel keeping the running 17-tap sums of c and c^2 (17 + 15 * 2 loads instead of
+// 16 * 17); 192 threads each walk one column of one of the six horizontal sums (17 + 7 * 2 loads instead of 8 * 17); every
+// pixel then reads its six window sums.
+// hp.img = last frame's temporal output (or prev_image), hp.aux = last frame's moments, of the rank that owns the row (PEER)
+template <bool PEER>
+__global__ void __launch_bounds__(256, 5) k_refl_temporal(GBufLevelDev cur, GBufLevelDev prev, const uint2* __restrict__ input, const HistPeers hp, FrameConsts fc,
+                                                        ReflTemporalParams P, uint2* __restrict__ out, uint2* __restrict__ mom_out, uint8_t* __restrict__ tile_flags)
+{
+    __shared__ float    s_c[3][24][49];  // row pitch 49: the 144 row walkers of a phase hit 32 different banks
+    __shared__ float    s_h[6][24][33];  // horizontal window sums: [ch] = sum c, [3 + ch] = sum c^2 (pitch 33: the row walkers store one column at a time)
+    __shared__ float    s_v[6][8][32];   // 17x17 window sums per pixel of the tile
+    __shared__ uint32_t s_flags;
+    const int W = cur.W, H = cur.H;
+    // PEER: the bottom halo rows read their history across NVLink (slow taps); they are scheduled first so that the bulk of the band
+    // covers their latency instead of leaving it as the kernel's tail
+    const int by = (int)blockIdx.y < P.rot ? (int)gridDim.y - P.rot + (int)blockIdx.y : (int)blockIdx.y - P.rot;
+    const int x0 = blockIdx.x * 32, y0 = P.row0 + by * 8;
+    const int lx = threadIdx.x & 31, ly = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_flags = 0;
+    for (int i = threadIdx.x; i < 48 * 24; i += 256)
     {
-        uint32_t t = ((b & 0xFFu) ? 1u : 0u) | ((b & 0xFF00u) ? 2u : 0u) | ((b & 0xFF0000u) ? 4u : 0u) | ((b & 0xFF000000u) ? 8u : 0u);
-        atomicOr(&s_flags, t);
+        const int rx = i % 48, ry = i / 48, px = x0 - 8 + rx, py = y0 - 8 + ry;
+        float     r = 0.0f, g = 0.0f, b = 0.0f;
+        if (inside(px, py, W, H))
+        {
+            const uint2  w = __ldg(input + (size_t)py * W + px);
+            const float2 a = h2_to_f2(w.x), c = h2_to_f2(w.y);
+            r = a.x; g = a.y; b = c.x;
+        }
+        s_c[0][ry][rx] = r; s_c[1][ry][rx] = g; s_c[2][ry][rx] = b;
     }
     __syncthreads();
-    if (threadIdx.x < 4)
-    {
-        const int tx = (x0 >> 3) + threadIdx.x, ty = y0 >> 3, TW = (W + 7) >> 3;
-        if (tx < TW && y0 < H && y0 < row1) tile_flags[(size_t)ty * TW + tx] = (s_flags >> threadIdx.x) & 1u;
+    if (threadIdx.x < 144)
+    { // horizontal: task = (half, channel, row); outputs 16 columns
+        const int    row = threadIdx.x % 24, ch = (threadIdx.x / 24) % 3, base = (threadIdx.x / 72) * 16;
+        const float* v = &s_c[ch][row][base];
+        float        a = 0.0f, b = 0.0f;
+#pragma unroll
+        for (int t = 0; t < 17; t++) { const float c = v[t]; a += c; b = fmaf(c, c, b); }
+        s_h[ch][row][base]     = a;
+        s_h[3 + ch][row][base] = b;
+#pragma unroll
+        for (int i = 1; i < 16; i++)
+        {
+            const float cin = v[16 + i], cout = v[i - 1];
+            a += cin - cout;
+            b = fmaf(cin, cin, fmaf(-cout, cout, b));
+            s_h[ch][row][base + i]     = a;
+            s_h[3 + ch][row][base + i] = b;
+        }
     }
+    __syncthreads();
+    if (threadIdx.x < 192)
+    { // vertical: task = (quantity, column); outputs 8 rows
+        const int    q = threadIdx.x >> 5, col = threadIdx.x & 31;
+        float        a = 0.0f;
+#pragma unroll
+        for (int r = 0; r < 17; r++) a += s_h[q][r][col];
+        s_v[q][0][col] = a;
+#pragma unroll
+        for (int i = 1; i < 8; i++)
+        {
+            a += s_h[q][16 + i][col] - s_h[q][i - 1][col];
+            s_v[q][i][col] = a;
+        }
+    }
+    __syncthreads();
+
+    const int x = x0 + lx, y = y0 + ly;
+    bool      flag = false;
+    if (x < W && y < H && y < P.row1)
+    {
+        const size_t idx   = (size_t)y * W + x;
+        const float  depth = __ldg(cur.depth + idx);
+        const uint2  g2w = __ldg(cur.gb2 + idx), g3w = __ldg(cur.gb3 + idx);
+        const float4 g2 = h4_to_f4(g2w), g3 = h4_to_f4(g3w);
+        const float  roughness = g3.x;
+        float        o[4] = { 0, 0, 0, 0 }, m[4] = { 0, 0, 0, 0 };
+        if (depth != 1.0f)
+        {
+            const float color[3] = { s_c[0][ly + 8][lx + 8], s_c[1][ly + 8][lx + 8], s_c[2][ly + 8][lx + 8] };
+            const float ray_length = h2_to_f2(__ldg(reinterpret_cast<const uint32_t*>(input + idx) + 1)).y;
+            const float fw = (float)W, fh = (float)H;
+            const float tu = ((float)x + 0.5f) / fw, tv = ((float)y + 0.5f) / fh;
+            const float3 cn = rn_octohedral_to_direction(g2.x, g2.y);
+            const float  cmesh = g3.z, curvature = g3.y;
+            const float3 cpos = rn_world_position_from_depth(tu, tv, depth, fc.view_proj_inverse);
+            // compute_history_coord, reprojection.glsl:101-111
+            float hfx = rn_mad(g2.z, fw, (float)x), hfy = rn_mad(g2.w, fh, (float)y);
+            if (ray_length > 0.0f && curvature == 0.0f)
+            { // virtual_point_reprojection :78-97 — exactly rounded: it lands on texel corners for a static camera
+                const float2 vp = rn_virtual_point_reprojection(x, y, fw, fh, depth, ray_length, fc.cam_pos, fc.view_proj_inverse, fc.prev_view_proj);
+                hfx = vp.x;
+                hfy = vp.y;
+            }
+            const int   hcx = (int)hfx, hcy = (int)hfy; // ivec2(reprojected_coord) :171
+            const float hu = __fadd_rn(tu, g2.z), hv = __fadd_rn(tv, g2.w);
+            const bool  in_frame = inside(hcx, hcy, W, H);
+            const HistOwner oc = owner_cache<PEER>(hp, max(hcy - 1, 0), min(hcy + 1, H - 1));
+            float hc[3] = { 0, 0, 0 }, hm0 = 0.0f, hm1 = 0.0f;
+            bool  valid = false;
+            if (in_frame)
+            {
+                const float fx = hfx - floorf(hfx), fy = hfy - floorf(hfy);
+                const float w4[4] = { (1 - fx) * (1 - fy), fx * (1 - fy), (1 - fx) * fy, fx * fy };
+                float sumw = 0.0f;
+                bool  any  = false;
+#pragma unroll
+                for (int s = 0; s < 4; s++)
+                {
+                    if (w4[s] == 0.0f) continue; // exact: see k_temporal
+                    const int px = hcx + (s & 1), py = hcy + (s >> 1);
+                    const HistTap t = fetch_prev(prev, px, py);
+                    if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                    {
+                        any = true;
+                        if (inside(px, py, W, H))
+                        {
+                            const size_t pi = (size_t)py * W + px;
+                            const float4 hv4 = h4_to_f4(hist_ld<PEER, uint2>(hp.img, hp, oc, py, pi));
+                            const float2 mm  = h2_to_f2(hist_ld<PEER, uint32_t>(hp.aux, hp, oc, py, 2 * pi));
+                            hc[0] += w4[s] * hv4.x; hc[1] += w4[s] * hv4.y; hc[2] += w4[s] * hv4.z;
+                            hm0 += w4[s] * mm.x; hm1 += w4[s] * mm.y;
+                        }
+                        sumw += w4[s];
+                    }
+                }
+                if (any)
+                {
+                    valid = sumw >= 0.01f;
+                    const float inv = valid ? fast_rcp(sumw) : 0.0f;
+                    hc[0] *= inv; hc[1] *= inv; hc[2] *= inv; hm0 *= inv; hm1 *= inv;
+                }
+                if (!valid)
+                {
+                    float cnt = 0.0f;
+                    for (int yy = -1; yy <= 1; yy++)
+                        for (int xx = -1; xx <= 1; xx++)
+                        {
+                            const int px = hcx + xx, py = hcy + yy;
+                            const HistTap t = fetch_prev(prev, px, py);
+                            if (rn_tap_valid(t, cpos, cn, cmesh, hu, hv, fc.view_proj_inverse))
+                            {
+                                if (inside(px, py, W, H))
+                                {
+                                    const size_t pi = (size_t)py * W + px;
+                                    const float4 hv4 = h4_to_f4(hist_ld<PEER, uint2>(hp.img, hp, oc, py, pi));
+                                    const float2 mm  = h2_to_f2(hist_ld<PEER, uint32_t>(hp.aux, hp, oc, py, 2 * pi));
+                                    hc[0] += hv4.x; hc[1] += hv4.y; hc[2] += hv4.z; hm0 += mm.x; hm1 += mm.y;
+                                }
+                                cnt += 1.0f;
+                            }
+                        }
+                    if (cnt > 0.0f) { valid = true; const float inv = fast_rcp(cnt); hc[0] *= inv; hc[1] *= inv; hc[2] *= inv; hm0 *= inv; hm1 *= inv; }
+                }
+            }
+            float hist_len = 0.0f;
+            if (valid) hist_len = h2_to_f2(hist_ld<PEER, uint32_t>(hp.aux, hp, oc, hcy, 2 * ((size_t)hcy * W + hcx) + 1)).x;
+            else { hc[0] = hc[1] = hc[2] = 0.0f; hm0 = hm1 = 0.0f; }
+            const float hlen = fminf(32.0f, valid ? hist_len + 1.0f : 1.0f);
+            if (valid)
+            { // clip_aabb(mean - sigma, mean + sigma) :111-129
+                float mn[3], mx[3];
+#pragma unroll
+                for (int ch = 0; ch < 3; ch++)
+                {
+                    const float m1 = s_v[ch][ly][lx], m2 = s_v[3 + ch][ly][lx];
+                    const float mean = m1 * (1.0f / 289.0f), var = m2 * (1.0f / 289.0f) - mean * mean, sd = sqrtf(fmaxf(var, 0.0f));
+                    mn[ch] = mean - sd;
+                    mx[ch] = mean + sd;
+                }
+                float cv[3], ctr[3], mabs = 0.0f;
+#pragma unroll
+                for (int ch = 0; ch < 3; ch++)
+                {
+                    ctr[ch] = 0.5f * (mx[ch] + mn[ch]);
+                    const float ext = 0.5f * (mx[ch] - mn[ch]) + 0.001f;
+                    cv[ch] = hc[ch] - ctr[ch];
+                    mabs   = fmaxf(mabs, fabsf(cv[ch] * fast_rcp(ext)));
+                }
+                if (mabs > 1.0f) { const float im = fast_rcp(mabs); hc[0] = ctr[0] + cv[0] * im; hc[1] = ctr[1] + cv[1] * im; hc[2] = ctr[2] + cv[2] * im; }
+            }
+            const float cdl = sqrtf(fc.camera_delta[0] * fc.camera_delta[0] + fc.camera_delta[1] * fc.camera_delta[1] + fc.camera_delta[2] * fc.camera_delta[2]);
+            const float maxacc = cdl > 0.0f ? 8.0f : hlen;
+            const float iacc   = fast_rcp(maxacc);
+            const float alpha  = valid ? fmaxf(P.alpha, iacc) : 1.0f;
+            const float alpham = valid ? fmaxf(P.moments_alpha, iacc) : 1.0f;
+            const float lum = luminance(color[0], color[1], color[2]);
+            const float mo0 = hm0 * (1.0f - alpham) + lum * alpham, mo1 = hm1 * (1.0f - alpham) + (lum * lum) * alpham;
+            o[0] = hc[0] * (1.0f - alpha) + color[0] * alpha;
+            o[1] = hc[1] * (1.0f - alpha) + color[1] * alpha;
+            o[2] = hc[2] * (1.0f - alpha) + color[2] * alpha;
+            o[3] = fmaxf(0.0f, mo1 - mo0 * mo0);
+            m[0] = mo0; m[1] = mo1; m[2] = hlen; m[3] = 0.0f;
+        }
+        mom_out[idx] = pack_h4(m[0], m[1], m[2], m[3]);
+        out[idx]     = pack_h4(o[0], o[1], o[2], o[3]);
+        flag = depth != 1.0f && roughness >= 0.05f && (P.approximate_with_ddgi != 1 || roughness <= 0.75f);
+    }
+    STORE_TILE_FLAGS(flag, s_flags, lx, x0, y0, W, H, P.row1, tile_flags);
 }
 
 } // namespace
@@ -348,4 +570,17 @@ void launch_temporal(int kind, const GBufLevelDev& cur, const GBufLevelDev& prev
     if (row1 <= row0) return;
     if (spp > 1) launch_temporal_form<true>(kind, cur, prev, { count, spp }, hist, fc, alpha, moments_alpha, out_img, out_aux, tile_flags, row0, row1, st);
     else launch_temporal_form<false>(kind, cur, prev, { mask }, hist, fc, alpha, moments_alpha, out_img, out_aux, tile_flags, row0, row1, st);
+}
+
+void launch_reflections_temporal(const GBufLevelDev& cur, const GBufLevelDev& prev, const void* input, const HistPeers& hist, const FrameConsts& fc, float alpha,
+                                 float moments_alpha, int approximate_with_ddgi, void* out, void* mom_out, uint8_t* tile_flags, int row0, int row1, cudaStream_t st)
+{
+    if (row1 <= row0) return;
+    dim3               grid((cur.W + 31) / 32, (row1 - row0 + 7) / 8);
+    int                rot = 0;
+    if (hist.world > 1 && hist.self < hist.world - 1) rot = (row1 - hist.band_end[hist.self] + 7) / 8; // tile rows below this rank's band
+    if (rot < 0 || rot >= (int)grid.y) rot = 0;
+    ReflTemporalParams P { alpha, moments_alpha, approximate_with_ddgi, row0, row1, rot };
+    if (hist.world > 1) k_refl_temporal<true><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
+    else k_refl_temporal<false><<<grid, 256, 0, st>>>(cur, prev, (const uint2*)input, hist, fc, P, (uint2*)out, (uint2*)mom_out, tile_flags);
 }
