@@ -104,6 +104,8 @@ __device__ float3 direct_lighting(const BvhDev& bvh, const hr_light& light, V3 W
         float  t_max, att;
         fetch_light_properties_hard(light, P, N, Li, Wi, t_max, att);
         const V3 Wh = det::normalize(det::add(Wo, Wi));
+        // evaluated before the shadow ray: only brdf, att and Li stay live across its traversal, not the surface and the directions
+        const float3 brdf = evaluate_uber_brdf(diffuse_color, roughness, N, F0, Wo, Wh, Wi);
         if (att > 0.0f)
         {
             sr.d    = Wi;
@@ -111,7 +113,6 @@ __device__ float3 direct_lighting(const BvhDev& bvh, const hr_light& light, V3 W
             count_rays(ray_ctr, 1, 1u);
             att *= trace_any(bvh, sr) ? 0.0f : 1.0f;
         }
-        const float3 brdf = evaluate_uber_brdf(diffuse_color, roughness, N, F0, Wo, Wh, Wi);
         Lo = Lo + (brdf * att) * Li;
     }
     if (sky_light)
@@ -296,10 +297,14 @@ struct ReflTraceParams { float bias, trim; int sample_gi, approximate_with_ddgi;
 // K12: warp = 8x4 pixel block (coherent reflection rays), 256 threads = 32x8 pixels
 // 2-warp CTAs (16x4 pixels): closest-hit rays + hit shading are heavy-tailed, small CTAs recycle their slots sooner (trace.cu)
 // MULTI = false: exactly the reference's one ray per pixel (straight-line code); true: the spp > 1 extension (sample loop)
-// MINB: resident 2-warp CTAs per SM the registers are tuned for; 18 (56 registers) for one ray per pixel.  Config 3 at 4K on an
-// H100 SXM 80 GB (400 W power limit), K12 per frame: 12 -> 3.15 ms, 14 -> 3.00, 16 -> 2.94, 18 -> 2.91, 20 -> 2.91: the kernel is
-// latency-bound, resident warps buy more than registers (and than the spills the smaller register budgets cost).
-template <bool MULTI, int MINB, bool TEX>
+// MINB: resident 2-warp CTAs per SM the registers are tuned for.  One ray per pixel: 24 (40 registers) without DDGI, 18 (56) with
+// it.  Config 3 at 4K on an H100 SXM 80 GB (700 W power limit), the GI = false kernel, K12 per frame: 16 -> 2.68 ms, 18 -> 2.61,
+// 20 -> 2.55, 24 -> 2.47: the kernel is latency-bound, resident warps buy more than registers (and than the spills the smaller
+// register budgets cost).
+// GI = false: sample_gi and approximate_with_ddgi are both off, so the kernel is compiled without the DDGI lookups and the IBL term
+// (IBL is only added with sample_gi); their live values would otherwise set the register allocation around the two traversals.
+// GI = true: both terms behind their run-time flags.
+template <bool MULTI, int MINB, bool TEX, bool GI>
 __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev g, BvhDev bvh, ShadeDev sd, FrameConsts fc, hr_ddgi_uniforms d, gi::AtlasDev at,
                                                                 ReflTraceParams P, const uint8_t* __restrict__ sobol, const uint8_t* __restrict__ srk,
                                                                 uint2* __restrict__ out, tex::TexDev T)
@@ -328,7 +333,8 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
     float  ray_length = -1.0f;
     // spp > 1 (SURVEY.md §8d): the GGX lobe draws spp directions, the clamped radiance is averaged, ray_length = first sample's
     const int  spp = MULTI ? (P.spp > 1 ? P.spp : 1) : 1;
-    const bool ggx = !(roughness < 0.05f) && !(roughness > 0.75f && P.approximate_with_ddgi == 1);
+    const bool approx_ddgi = GI && P.approximate_with_ddgi == 1, gi_on = GI && P.sample_gi == 1;
+    const bool ggx = !(roughness < 0.05f) && !(roughness > 0.75f && approx_ddgi);
     const int  n_s = MULTI ? (ggx ? spp : 1) : 1;
     float3     acc = make_float3(0, 0, 0);
 #pragma unroll 1
@@ -336,7 +342,7 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
     {
         bool trace = false;
         if (roughness < 0.05f) { r.d = reflect(det::scale(Wo, -1.0f), N); trace = true; }
-        else if (roughness > 0.75f && P.approximate_with_ddgi == 1)
+        else if (roughness > 0.75f && approx_ddgi)
         {
             const V3 R = reflect(det::scale(Wo, -1.0f), N);
             using namespace gi;
@@ -358,8 +364,8 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
             count_rays(fc.ray_ctr, 0, 1u);
             if (trace_closest(bvh, r, t, prim, hu, hv))
             {
-                color = TEX ? shade_hit_tex(bvh, sd, T, fc.light, r, prim, hu, hv, false, 0.0f, 0.0f, sky, P.sample_gi == 1, d, at, P.gi_intensity, fc.ray_ctr, P.ibl)
-                            : shade_hit(bvh, sd, fc.light, r, prim, hu, hv, false, 0.0f, 0.0f, sky, P.sample_gi == 1, d, at, P.gi_intensity, fc.ray_ctr, P.ibl);
+                color = TEX ? shade_hit_tex(bvh, sd, T, fc.light, r, prim, hu, hv, false, 0.0f, 0.0f, sky, gi_on, d, at, P.gi_intensity, fc.ray_ctr, P.ibl)
+                            : shade_hit(bvh, sd, fc.light, r, prim, hu, hv, false, 0.0f, 0.0f, sky, gi_on, d, at, P.gi_intensity, fc.ray_ctr, P.ibl);
                 if (s == 0) ray_length = 0.001f + t;
             }
             else color = sky;
@@ -611,16 +617,19 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
     if (d) du = *d;
     gi::AtlasDev at { (const uint2*)irr, (const uint32_t*)depth };
     const bool textured = sc->tex.n_textures > 0; // material textures: the TEX instantiations
+    const bool gi = sample_gi == 1 || approximate_with_ddgi == 1; // the spp > 1 kernels keep both terms behind their flags
     dim3 grid((g.W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
     const tex::TexDev& T = sc->tex;
 #define HR_K12_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, du, at, P, sobol, srk, (uint2*)out, T
     if (textured)
     {
-        if (spp > 1) k_reflections_ray_trace<true, 8, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-        else k_reflections_ray_trace<false, 18, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+        if (spp > 1) k_reflections_ray_trace<true, 8, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+        else if (gi) k_reflections_ray_trace<false, 18, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+        else k_reflections_ray_trace<false, 24, true, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
     }
-    else if (spp > 1) k_reflections_ray_trace<true, 8, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else k_reflections_ray_trace<false, 18, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+    else if (spp > 1) k_reflections_ray_trace<true, 8, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+    else if (gi) k_reflections_ray_trace<false, 18, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+    else k_reflections_ray_trace<false, 24, false, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
 #undef HR_K12_ARGS
 }
 

@@ -95,8 +95,10 @@ __device__ __forceinline__ SlabSetup slab_setup(const Ray& r)
 __device__ __forceinline__ void node_test(const float4* __restrict__ nodes, int node, const SlabSetup& s, float tmin, float tmax, bool& h0, bool& h1,
                                           float& tn0, float& tn1, int& c0, int& c1)
 {
-    // The 64-byte node is fetched with four 128-bit loads issued back to back (volatile asm): the child indices are loaded
-    // up front, so the scheduler cannot sink them below the box tests (a second L1 round trip per traversal step otherwise).
+    // The 64-byte node is fetched with four 128-bit loads (volatile asm).  ptxas still narrows the last one to the two link
+    // words (the upper 8 bytes are padding) and issues it after the box test's branch, where the links are first used: a
+    // second L1 round trip per step whose box test passes.  A branch-free step that consumes the links in the test's block
+    // issues it with the boxes, but measured slower (DESIGN.md §8).
     const float4* np = nodes + 4ull * node;
     float4        n0, n1, nz;
     int           pad0, pad1;
