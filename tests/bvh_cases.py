@@ -100,6 +100,86 @@ def chain(n):
     return _f32(out)
 
 
+def random_soup(n, seed=0, extent=10.0, size=1.0):
+    """n triangles of random orientation and size up to `size`, centred uniformly in a cube of side `extent`"""
+    rng = np.random.default_rng(seed)
+    c = rng.uniform(0.0, extent, (n, 1, 3))
+    return _f32((c + rng.uniform(-0.5, 0.5, (n, 3, 3)) * size * rng.uniform(0.05, 1.0, (n, 1, 1))).reshape(n, 9))
+
+
+def clustered(n_clusters=8, per=64, seed=0):
+    """Gaussian clusters of small triangles, cluster sizes and spreads varying, far apart from each other"""
+    rng = np.random.default_rng(seed)
+    out = []
+    for _ in range(n_clusters):
+        c = rng.uniform(0.0, 100.0, 3)
+        s = 10.0 ** rng.uniform(-1, 1)
+        out.append(c + rng.normal(0.0, s, (per, 1, 3)) + rng.uniform(-0.2, 0.2, (per, 3, 3)) * s)
+    return _f32(np.concatenate(out).reshape(-1, 9))
+
+
+def strip(quads=512):
+    """a long planar strip of unit quads along x in the plane y = 0, two triangles each"""
+    out = []
+    for i in range(quads):
+        out.append([i, 0, 0, i + 1, 0, 0, i + 1, 0, 1])
+        out.append([i, 0, 0, i + 1, 0, 1, i, 0, 1])
+    return _f32(out)
+
+
+def far_pairs(n, size=0.01, spacing=100.0):
+    """n // 2 pairs of small triangles (side `size`), the two of a pair about a unit apart and the pairs `spacing` apart
+    (plus one more triangle for odd n): the cheapest trees keep a pair as an internal node over two one-triangle leaves,
+    since one leaf of both would be tested by every ray that enters the pair's long box"""
+    tri = np.array([0.0, 0.0, 0.0, size, 0.0, 0.0, 0.0, size, size])
+    return _f32([tri + np.tile([spacing * (k // 2) + (k % 2), 0.5 * (k % 2), 0.25 * (k % 2)], 3) for k in range(n)])
+
+
+def points_and_segments(n, seed=0):
+    """zero-area boxes: points (three equal vertices, every other one twice) and segments along an axis, at random places.
+    Two copies of a point cost 0 as one leaf and 0 as an inner node: the build packs them as a leaf (ties go to the leaf)."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for k in range(n):
+        p = out[-2][:3] if k % 4 == 2 else rng.uniform(0.0, 8.0, 3)
+        if k % 2 == 0:
+            out.append(np.concatenate([p, p, p]))
+        else:
+            e = np.eye(3)[int(rng.integers(0, 3))] * rng.uniform(0.1, 3.0)
+            out.append(np.concatenate([p, p + e, p + 0.5 * e]))
+    return _f32(out)
+
+
+def deep_chain_cluster():
+    """chain(62) and five small triangles among its lowest ones, found by a search with the treelet restatement
+    (bvh_treelet.py): plain PLOC builds it exactly MAX_DEPTH deep (DEEP_CHAIN_CLUSTER_PLOC), and the cheapest treelet at the
+    chain's bottom would take a triangle one level deeper, so the restructuring's depth guard has to refuse it"""
+    cluster = [
+        [0.6619769930839539, -0.43171611428260803, 1.9393442869186401, 0.5848695039749146, -0.4460156559944153, 1.896966814994812,
+         0.599098801612854, -0.550525963306427, 1.941376805305481],
+        [2.0024828910827637, 0.25815069675445557, 0.11551348865032196, 2.6716103553771973, 0.07642986625432968, 0.5076364278793335,
+         2.725355625152588, 0.25231078267097473, 0.3219222128391266],
+        [2.295197010040283, 1.3277125358581543, 0.004972369875758886, 1.9215171337127686, 1.5196951627731323, 0.023755604401230812,
+         2.0728631019592285, 1.2457642555236816, -0.11852587759494781],
+        [1.1302663087844849, -0.001505021471530199, -0.006700961850583553, 1.1840806007385254, 0.08699750900268555,
+         -0.015070694498717785, 1.2224746942520142, -0.05395051836967468, 0.12170501053333282],
+        [0.6048675179481506, 1.1207380294799805, 0.28542760014533997, 0.6170430779457092, 1.113888144493103, 0.2835697531700134,
+         0.6057540774345398, 1.1093798875808716, 0.28516000509262085],
+    ]
+    return np.ascontiguousarray(np.concatenate([chain(62), _f32(cluster)]))
+
+
+def _deep_chain_cluster_ploc():
+    t = (((("leaf", 65, 66), 62), 0), ((("leaf", 63, 64), 1), 2))
+    for k in range(3, 62):
+        t = (t, k)
+    return t
+
+
+# plain PLOC's tree of deep_chain_cluster() in bvh_treelet.ordered form (primitive ids; ("leaf", a, b) is a packed leaf)
+DEEP_CHAIN_CLUSTER_PLOC = _deep_chain_cluster_ploc()
+
+
 def scene_bounds(tri):
     v = tri.reshape(-1, 3).astype(np.float64)
     return v.min(0), v.max(0)
