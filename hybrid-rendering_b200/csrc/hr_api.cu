@@ -1391,3 +1391,4 @@ int hr_shard_config(hr_ctx* ctx, int rank, int world)
 
 #include "hr_api_gi.inc"
 #include "hr_api_post.inc"
+#include "hr_api_reference.inc"

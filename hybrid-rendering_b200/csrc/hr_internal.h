@@ -187,7 +187,7 @@ struct hr_scene {
     hr_scene_info info {};
 };
 
-enum PassKind { PASS_SHADOWS = 1, PASS_AO = 2, PASS_REFLECTIONS = 3, PASS_DDGI = 4, PASS_DEFERRED = 5, PASS_TAA = 6, PASS_TONEMAP = 7, PASS_PATH_TRACER = 8 };
+enum PassKind { PASS_SHADOWS = 1, PASS_AO = 2, PASS_REFLECTIONS = 3, PASS_DDGI = 4, PASS_DEFERRED = 5, PASS_TAA = 6, PASS_TONEMAP = 7, PASS_PATH_TRACER = 8, PASS_REFERENCE = 9 };
 
 struct StageTimer { // one Rec per profiled render; hr_pass_stage_times averages and recycles them
     struct Rec { std::vector<std::string> names; std::vector<cudaEvent_t> ev; };
@@ -250,6 +250,16 @@ struct hr_pass {
     uint32_t  pt_frame_idx = 0;                        // GroundTruthPathTracer::m_frame_idx
     int       pt_ping_pong = 0;                        // GroundTruthPathTracer::m_ping_pong
     std::vector<void*> ddgi_grid_allocs;
+    // reference (hr_reference_create): the pass it references, that pass's kind, the samples accumulated per pixel of its rows, the accumulators
+    // (shadows / AO: unoccluded rays; reflections: float64 sum and sum of squares per channel) and the MEAN / STDERR images
+    hr_pass*  ref_target = nullptr;
+    int       ref_kind = 0;
+    uint32_t  ref_samples = 0;
+    int       ref_rows[2] = { 0, 0 };   // the rows every render since the last reset covers
+    uint32_t* ref_count = nullptr;
+    double*   ref_acc = nullptr;
+    uint8_t*  ref_mean = nullptr;
+    uint8_t*  ref_err = nullptr;
     // linked DDGI (shard.cu): the peers' atlas addresses as this rank sees them ([rank][irradiance 0, 1, depth 0, 1], shared image 0), the
     // frame tick of the render that published this rank's current atlases (0: not yet), the IPC mappings of the peers' atlases, the replaced
     // atlases of an IPC rank until the next handle exchange (the peers map them), and the pool same-process ranks allocate their grids from
@@ -299,6 +309,16 @@ void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, con
                                   float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
                                   const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
                                   int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st); // chunk_stride > 1: only the 8-row chunks c = chunk_first + i * chunk_stride (rows are ignored)
+
+// reference.cu (hr_reference_render): samples k0 .. k0 + n - 1 of rows [row0, row1) of the full-resolution G-buffer level g
+void launch_reference_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, uint32_t k0, int n, int row0, int row1,
+                           uint32_t* count, cudaStream_t st); // kind PASS_SHADOWS (K1: p0 = bias) or PASS_AO (K7: p0 = ray length, p1 = bias)
+void launch_reference_reflections(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
+                                  const hr_reflections_params& prm, int sample_gi, int approximate_with_ddgi, const void* brdf_lut, uint32_t k0, int n, int row0,
+                                  int row1, double* acc, cudaStream_t st);
+// MEAN (R16F from count, or RGBA16F from acc) and STDERR of rows [row0, row1) after n_samples samples
+void launch_reference_resolve(const GBufLevelDev& g, const uint32_t* count, const double* acc, uint32_t n_samples, float sky_value, float power, int row0, int row1,
+                              void* mean, void* err, cudaStream_t st);
 
 // ---- row-band sharding (shard.cu) ---------------------------------------------------------------------
 // An image whose rows are owned band-wise by the ranks.  The band partition is defined on the PASS height `H`

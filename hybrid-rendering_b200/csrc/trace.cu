@@ -11,7 +11,7 @@
 // Mapping: one warp = one 8x4 pixel block = one mask word (bit = lane = (y&3)*8 + (x&7), exactly
 // gl_LocalInvocationIndex of the reference's 8x4 workgroup), so the word is a single __ballot_sync.
 
-#include "traverse.cuh"
+#include "mask_px.cuh"
 #include <type_traits>
 
 namespace {
@@ -58,22 +58,7 @@ __device__ __forceinline__ uint32_t trace_pixel(const GBufLevelDev& g, const Bvh
                 const float r0 = det::sample_blue_noise(x, y, si, 0, sobol, sr);
                 const float r1 = det::sample_blue_noise(x, y, si, 1, sobol, sr);
                 Ray         r;
-                r.tmin = 0.01f;
-                if (MODE == 0)
-                {
-                    r.o = det::add(P, det::scale(N, p0)); // bias
-                    float att;
-                    det::fetch_light_properties_shadow(fc.light, P, N, r0, r1, r.d, r.tmax, att);
-                    if (att > 0.0f) { add_traced(traced); n += trace_any(bvh, r) ? 0u : 1u; }
-                }
-                else
-                {
-                    r.o    = det::add(P, det::scale(N, p1)); // bias
-                    r.d    = det::sample_cosine_lobe(N, r0, r1);
-                    r.tmax = p0; // ray_length
-                    add_traced(traced);
-                    n += trace_any(bvh, r) ? 0u : 1u;
-                }
+                if (mask_ray<MODE>(fc, P, N, p0, p1, r0, r1, r)) { add_traced(traced); n += trace_any(bvh, r) ? 0u : 1u; }
             }
         }
     }

@@ -134,7 +134,7 @@ ABI_SYMBOLS = [
     "hr_ddgi_default_params", "hr_ddgi_create", "hr_ddgi_render", "hr_ddgi_get_uniforms", "hr_reflections_default_params", "hr_reflections_create",
     "hr_reflections_render", "hr_pass_get_stats", "hr_pass_output_checksum", "hr_gbuffer_render", "hr_gbuffer_render_sharded", "hr_brdf_lut_set", "hr_deferred_create", "hr_deferred_render", "hr_gbuffer_stage_render", "hr_bluenoise_set_slot",
     "hr_taa_default_params", "hr_taa_jitter", "hr_taa_create", "hr_taa_render", "hr_tonemap_default_params", "hr_tonemap_create", "hr_tonemap_render", "hr_path_tracer_default_params", "hr_path_tracer_create", "hr_path_tracer_render", "hr_scene_set_textures",
-    "hr_compare_default_params", "hr_compare_sums_add", "hr_compare_finish", "hr_image_compare",
+    "hr_compare_default_params", "hr_compare_sums_add", "hr_compare_finish", "hr_image_compare", "hr_reference_create", "hr_reference_render",
 ]
 
 _product = None
@@ -796,3 +796,25 @@ class PathTracerPass(Pass):
 
     def render(self, frame: hr_frame, stream=0):
         self.ctx.check(self.lib.hr_path_tracer_render(self.h, C.byref(frame), C.byref(self.params), C.c_void_p(stream)), "hr_path_tracer_render")
+
+
+REFERENCE_OUT_STDERR = 1
+REFERENCE_OUT_MEAN = 100
+
+
+class ReferencePass(Pass):
+    """converged reference of a shadows, AO or reflections pass (hr_reference_*): render(frame, samples) adds `samples` rays per pixel
+    with the target's ray function and parameters (`params`, by default the target's own block); download(REFERENCE_OUT_MEAN) is the
+    mean through the target FINAL's per-pixel transform, download(REFERENCE_OUT_STDERR) its standard error; reset_history() restarts"""
+
+    def __init__(self, target: Pass):
+        self.ctx, self.kind, self.lib = target.ctx, "reference", target.lib
+        self.target = target
+        h = C.c_void_p()
+        self.ctx.check(self.lib.hr_reference_create(target.h, C.byref(h)), "hr_reference_create")
+        self.h = h
+
+    def render(self, frame: hr_frame, samples, params=None, ddgi: DDGIPass = None, row0=0, row1=0, stream=0):
+        prm = params if params is not None else self.target.params
+        self.ctx.check(self.lib.hr_reference_render(self.h, C.byref(frame), C.byref(prm), ddgi.h if ddgi is not None else None, int(samples), int(row0), int(row1),
+                                                    C.c_void_p(stream)), "hr_reference_render")

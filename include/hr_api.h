@@ -538,6 +538,52 @@ HR_API int  hr_path_tracer_create(hr_ctx* ctx, int width, int height, hr_pass** 
 HR_API int  hr_path_tracer_render(hr_pass* pass, const hr_frame* frame, const hr_path_tracer_params* params, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Converged references of the shadows, AO and reflections signals (reference.cu, DESIGN.md §8)
+ *
+ * A reference pass estimates the signal its target pass denoises: the same G-buffer, the same per-ray function (K1's soft-shadow
+ * ray, K7's cosine-lobe ray, K12's mirror / DDGI / GGX sample with its shading and its 0.7 clamp) and the same parameters, averaged
+ * over many independent rays per pixel instead of denoised from one.  The difference between the target's FINAL output and the
+ * reference's MEAN is then the error of the denoise chain alone.
+ *
+ * Only the random numbers differ from the target's ray trace: (r0, r1) of sample k at pixel (x, y) are the first two next_float of
+ * the xoroshiro64* stream of the path tracer seeded with rng_init(x, y, k) (random.glsl), not the 256-periodic blue noise.  Sample
+ * k is the k-th sample the pass has accumulated, so any split of the samples over renders traces the same rays: shadows and AO
+ * counts are identical, reflection sums equal up to float64 rounding.
+ *
+ * Output at the target's FINAL resolution (the full resolution, whatever the target's scale), the signal alone:
+ *   HR_REFERENCE_OUT_MEAN    R16F (shadows, AO) or RGBA16F (rgb, 1) (reflections): the accumulated mean passed through the per-pixel
+ *                            transform the target's FINAL applies after filtering, read from the parameters: shadows raise it to
+ *                            `power` when denoise is on and filter_iterations >= 1 (the last a-trous iteration), AO when denoise is
+ *                            on and the target's scale is not FULL (the upsample); reflections apply none.  Sky pixels (depth 1)
+ *                            hold the FINAL's sky value: 0 for shadows, 1 for AO, (0, 0, 0, 1) for reflections.
+ *   HR_REFERENCE_OUT_STDERR  same format: the standard error of the untransformed mean per channel, sqrt(s^2 / N) with the unbiased
+ *                            sample variance s^2 of the N samples (0 for N = 1 and at sky pixels).  Mirror and DDGI-branch reflection
+ *                            pixels do not depend on the sample: their STDERR is 0.
+ * A shadows target at full resolution has an RG16F FINAL (visibility, variance): compare its r channel, copied into an R16F
+ * image, with MEAN (hr_image_compare takes images of one format).
+ *
+ * Accumulation: one sample counter N for the rendered rows (uint32, restarted by hr_pass_reset_history, which the caller calls when the
+ * view, the scene or the light changes: the reference does no reprojection).  Shadows and AO keep a uint32 count of unoccluded rays
+ * per pixel, reflections float64 sums of the value and of its square per channel.  hr_pass_get_stats counts the rays traced (the
+ * mirror and DDGI-branch samples are evaluated once per render); hr_pass_output, the downloads, the checksum and hr_pass_destroy
+ * work as for any pass.  The target must outlive its reference.
+ * ---------------------------------------------------------------------------------------------- */
+enum { HR_REFERENCE_OUT_STDERR = 1, HR_REFERENCE_OUT_MEAN = 100 };
+/* A reference of `target` (a shadows, AO or reflections pass); HR_ERR_INVALID_ARG for a pass of another kind. */
+HR_API int hr_reference_create(hr_pass* target, hr_pass** out);
+/* Adds `samples` (1..65536) rays per pixel on rows [row0, row1) (row1 <= 0: to the last row) of the current G-buffer slot
+ * (frame->ping_pong) at mip 0, then writes MEAN and STDERR of those rows; the other rows are left as they are.  The one sample
+ * counter N counts the samples of these rows, so every render between two resets covers the same rows: a render over other rows
+ * than the first one after the reset is refused.  A sharded rank renders its band and the 5 rows beyond it that the SSIM window
+ * of hr_image_compare reads.
+ * params: the target's parameter block (hr_shadows_params, hr_ao_params or hr_reflections_params).  ddgi: reflections only, may be
+ * NULL; the DDGI and IBL terms are switched on exactly as hr_reflections_render decides for the target's next render with that
+ * DDGI pass (off on the target's first frame, so render the reference before the target in that frame).
+ * HR_ERR_INVALID_ARG, changing nothing: NULL pointers, a bad sample count or row range, rows other than those of the first render
+ * since the reset, N passing 2^32 - 1, non-finite parameters, or a DDGI pass of another context. */
+HR_API int hr_reference_render(hr_pass* ref, const hr_frame* frame, const void* params, hr_pass* ddgi, int samples, int row0, int row1, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Common pass functions
  * ---------------------------------------------------------------------------------------------- */
 /* output_ds() equivalent: borrowed device image, valid until the next render/destroy of this pass. */
