@@ -218,6 +218,13 @@ int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, co
         const hr_instance& in = instances[ii];
         const float*       M  = in.model;
         if ((size_t)in.first_index + in.index_count > n_indices) { hr_set_error(ctx, "hr_scene_build: instance %zu index range out of bounds", ii); return HR_ERR_INVALID_ARG; }
+        // every shading kernel reads d_materials[prim_mat] (and, with textures, TexDev::mat[prim_mat]) unchecked; a scene without materials
+        // (shadows and AO only) is legal and refused by the shading renders instead
+        if (n_materials > 0 && in.material_idx >= n_materials)
+        {
+            hr_set_error(ctx, "hr_scene_build: instance %zu material_idx %u out of range (%zu materials)", ii, in.material_idx, n_materials);
+            return HR_ERR_INVALID_ARG;
+        }
         for (uint32_t k = 0; k + 2 < in.index_count; k += 3)
         {
             float tb[18];

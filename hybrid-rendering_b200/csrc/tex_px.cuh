@@ -46,6 +46,14 @@ HR_TEX_HD int tex_f2i(float f)
     return (int)f;
 #endif
 }
+HR_TEX_HD int next_texel(int i)
+{ // i + 1; a saturated x0 = INT_MAX wraps to INT_MIN like the device's 32-bit add (signed overflow is undefined in host C++)
+#ifdef __CUDA_ARCH__
+    return i + 1;
+#else
+    return (int)((uint32_t)i + 1u);
+#endif
+}
 HR_TEX_HD int wrap_repeat(int i, int n) { const int m = i % n; return m < 0 ? m + n : m; } // VK_SAMPLER_ADDRESS_MODE_REPEAT
 
 HR_TEX_HD RGBA fetch(const TexDev& T, const TexDesc& d, int x, int y)
@@ -66,7 +74,8 @@ HR_TEX_HD RGBA sample(const TexDev& T, int ti, float u, float v)
     const float fx0 = floorf(x), fy0 = floorf(y);
     const float fx = x - fx0, fy = y - fy0;
     const int   x0 = tex_f2i(fx0), y0 = tex_f2i(fy0);
-    const RGBA  a = fetch(T, d, x0, y0), b = fetch(T, d, x0 + 1, y0), c = fetch(T, d, x0, y0 + 1), e = fetch(T, d, x0 + 1, y0 + 1);
+    const int   x1 = next_texel(x0), y1 = next_texel(y0);
+    const RGBA  a = fetch(T, d, x0, y0), b = fetch(T, d, x1, y0), c = fetch(T, d, x0, y1), e = fetch(T, d, x1, y1);
     const float wx0 = 1.0f - fx, wy0 = 1.0f - fy;
     RGBA r;
     r.r = (a.r * wx0 + b.r * fx) * wy0 + (c.r * wx0 + e.r * fx) * fy;

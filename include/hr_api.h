@@ -146,7 +146,9 @@ typedef struct hr_instance {
  * fit (hr_debug_set key 3), collapsed into <= 2-triangle leaves and packed into 64-byte two-child nodes.  Host pointers in; synchronises the context's build
  * stream before returning.  Fails with HR_ERR_UNSUPPORTED when the tree is deeper than the traversal stack (64).  Every
  * built scene gets a new process-wide serial number; a DDGI pass re-initialises its probe grid when it next renders a scene
- * with another serial, even one allocated at a destroyed scene's address. */
+ * with another serial, even one allocated at a destroyed scene's address.  With n_materials > 0, an instance whose material_idx
+ * is not below n_materials is refused with HR_ERR_INVALID_ARG before anything is allocated.  A scene built without materials
+ * (n_materials = 0) serves the shadows and AO passes only: every render that shades hits refuses it with HR_ERR_NOT_READY. */
 HR_API int hr_scene_build(hr_ctx* ctx, const hr_vertex* vertices, size_t n_vertices, const uint32_t* indices, size_t n_indices,
                           const hr_instance* instances, size_t n_instances, const hr_material* materials, size_t n_materials,
                           hr_scene** out);
@@ -534,7 +536,8 @@ enum {
 HR_API void hr_path_tracer_default_params(hr_path_tracer_params* p);
 HR_API int  hr_path_tracer_create(hr_ctx* ctx, int width, int height, hr_pass** out);
 /* render(), ground_truth_path_tracer.cpp:44-113: the sample index is the pass's own counter (m_frame_idx, push constant num_frames),
- * restarted by hr_pass_reset_history (restart_accumulation(), ground_truth_path_tracer.h:17). */
+ * restarted by hr_pass_reset_history (restart_accumulation(), ground_truth_path_tracer.h:17).  HR_ERR_NOT_READY without a current
+ * scene or when the current scene was built without materials. */
 HR_API int  hr_path_tracer_render(hr_pass* pass, const hr_frame* frame, const hr_path_tracer_params* params, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

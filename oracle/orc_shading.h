@@ -77,7 +77,9 @@ struct Texture2D {
         float i0 = floorf(x), j0 = floorf(y);
         float a = x - i0, b = y - j0;
         int   i = f2i(i0), j = f2i(j0);
-        vec4  t00 = texel(i, j), t10 = texel(i + 1, j), t01 = texel(i, j + 1), t11 = texel(i + 1, j + 1);
+        // the neighbour of a saturated index (|u * W| >= 2^31) wraps to INT_MIN, as a GPU's 32-bit add does; written unsigned (no signed overflow)
+        int   i1 = (int)((uint32_t)i + 1u), j1 = (int)((uint32_t)j + 1u);
+        vec4  t00 = texel(i, j), t10 = texel(i1, j), t01 = texel(i, j1), t11 = texel(i1, j1);
         auto  lerp2 = [&](float p, float q, float r, float s) { return (p * (1.0f - a) + q * a) * (1.0f - b) + (r * (1.0f - a) + s * a) * b; };
         return { lerp2(t00.x, t10.x, t01.x, t11.x), lerp2(t00.y, t10.y, t01.y, t11.y), lerp2(t00.z, t10.z, t01.z, t11.z), lerp2(t00.w, t10.w, t01.w, t11.w) };
     }

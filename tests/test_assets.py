@@ -707,3 +707,22 @@ def test_png_encode_decode_property(tmp_path):
 
     ours()
     theirs()
+
+
+@pytest.mark.parametrize("fmt", ["obj", "gltf", "glb"])
+def test_scene_material_indices_are_in_range(tmp_path, fmt):
+    """hr_scene_build refuses an instance whose material_idx is not below n_materials: neither the scene tables of loaded meshes (each
+    mesh's sub-mesh indices offset by its first material, meshes instanced more than once) nor the synthetic scenes produce one"""
+    sc = pyhr.SynthScene(pyhr.SCENE_SHADOWS_TEST)
+    path, models = export_obj(sc, tmp_path) if fmt == "obj" else export_gltf(sc, tmp_path, glb=(fmt == "glb"))
+    (tmp_path / "cube.obj").write_text(OBJ_TEXT)
+    (tmp_path / "cube.mtl").write_text(MTL_TEXT)
+    mesh, cube = A.Mesh(path), A.Mesh(tmp_path / "cube.obj")
+    ident = np.eye(4, dtype=np.float32).reshape(-1)
+    asc = A.AssetScene([(cube, ident), (mesh, models[0]), (cube, ident), (mesh, models[1])])
+    idx = [i["material_idx"] for i in asc.instances()]
+    assert asc.n_materials == cube.n_materials + mesh.n_materials and max(idx) == asc.n_materials - 1 and min(idx) == 0
+    for kind in (pyhr.SCENE_SHADOWS_TEST, pyhr.SCENE_ARCADE):
+        s = pyhr.SynthScene(kind, 2000)
+        _, _, insts, mats = synth_arrays(s)
+        assert max(it.material_idx for it in insts) < len(mats)

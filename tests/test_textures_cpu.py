@@ -85,15 +85,29 @@ def test_sampler_closed_forms():
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_device_sampler_equals_the_oracle_bit_for_bit(seed):
     rng = np.random.default_rng(seed)
-    textures = [(rng.integers(0, 256, (5, 7, 4), dtype=np.uint8), True), (rng.integers(0, 256, (16, 16), dtype=np.uint8), False),
-                (rng.integers(0, 256, (3, 2, 2), dtype=np.uint8), False), (rng.integers(0, 256, (1, 1, 4), dtype=np.uint8), True),
-                (rng.integers(0, 256, (64, 33, 4), dtype=np.uint8), False)]
+    r = lambda *shape: rng.integers(0, 256, shape, dtype=np.uint8)  # noqa: E731
+    textures = [(r(5, 7, 4), True), (r(16, 16), False), (r(3, 2, 2), False), (r(1, 1, 4), True), (r(64, 33, 4), False),
+                # 1 x N, N x 1, NPOT sizes, the widest accepted image; sRGB on 1- and 2-channel images
+                (r(9, 1, 4), False), (r(1, 11, 4), True), (r(5, 3, 4), True), (r(13, 7), True), (r(17, 33, 2), True), (r(1, 16384, 4), False)]
     texels, desc = pack(textures)
     lut = srgb_lut()
     L = emu()
-    uv = np.concatenate([rng.uniform(-3, 4, (4000, 2)), rng.uniform(-1e4, 1e4, (200, 2)),
+    base = rng.uniform(-3, 4, (4000, 2))
+    borders = []
+    for img, _ in textures:  # texel borders and centres of every size, and their float neighbours on both sides
+        h, w = img.shape[:2]
+        for n in (w, h):
+            c = np.concatenate([np.arange(-n, 2 * n + 1) / n, (np.arange(-n, 2 * n + 1) + 0.5) / n]).astype(np.float32)
+            borders.append(np.concatenate([c, np.nextafter(c, np.float32(-np.inf)), np.nextafter(c, np.float32(np.inf))]))
+    borders = np.concatenate(borders)
+    uv = np.concatenate([base, rng.uniform(-1e4, 1e4, (200, 2)),
                          np.stack(np.meshgrid(np.arange(-8, 9) / 7.0, np.arange(-8, 9) / 5.0), -1).reshape(-1, 2),          # exact texel borders of the 7 x 5 image
-                         np.stack(np.meshgrid((np.arange(-8, 9) + 0.5) / 16.0, (np.arange(-8, 9) + 0.5) / 16.0), -1).reshape(-1, 2)]).astype(np.float32)
+                         np.stack(np.meshgrid((np.arange(-8, 9) + 0.5) / 16.0, (np.arange(-8, 9) + 0.5) / 16.0), -1).reshape(-1, 2),
+                         rng.choice(borders, (3000, 2)),
+                         base[:600] + np.array([[4096.0, -4096.0]]), base[600:1200] + np.array([[-8191.0, 8191.0]]),                 # integer offsets
+                         rng.uniform(1e5, 1e7, (400, 2)) * rng.choice([-1.0, 1.0], (400, 2)),                                      # few fraction bits
+                         rng.uniform(2.2e9, 1e12, (300, 2)) * rng.choice([-1.0, 1.0], (300, 2)),                                    # |u W| >= 2^31 for W >= 1
+                         rng.uniform(1.4e5, 1e8, (300, 2)) * rng.choice([-1.0, 1.0], (300, 2))]).astype(np.float32)                # >= 2^31 for the 16384-wide image
     for ti, (img, srgb) in enumerate(textures):
         want = O.texture_sample(img, srgb, uv)
         got = np.empty_like(want)
@@ -251,3 +265,47 @@ def test_oracle_gbuffer_and_path_tracer_see_the_textures():
     assert np.array_equal(p0.prim, p1.prim) and not np.array_equal(a, b)
     tex.set_textures([], [], np.zeros((0, 6), np.float32))  # removing them restores the constants
     assert np.array_equal(O.gbuffer_render(tex, f, W, H).gb1, g0.gb1)
+
+
+@pytest.mark.parametrize("case", ["far_uv", "texel_borders", "sizes", "many", "channels", "normal_maps"])
+def test_device_fetch_on_the_edge_cases_equals_the_oracle(case):
+    """material_at_hit and normal_at_hit (both call sites) of the host build against the oracle on the scenes of texture_cases.py:
+    coordinates far from the origin and on texel borders, every size, 300 textures and materials, channels 0..3, normal maps with zero
+    tangents; bit for bit, NaNs compared by class"""
+    import texture_cases as TC
+    c = TC.build(case)
+    ss = O.ShadingScene(c.sc, brute=True)
+    vuv, vtb = c.vuv(), c.vtb()
+    ss.set_textures(c.textures, c.bindings, vuv, vtb)
+    rng = np.random.default_rng(11)
+    n = 8000
+    prim = rng.integers(0, c.sc.n_tris, n).astype(np.uint32)
+    bu = rng.random(n).astype(np.float32)
+    bary = np.stack([bu, (rng.random(n).astype(np.float32) * (1.0 - bu)).astype(np.float32)], -1)
+    bary[:50] = 0.0  # exactly on corner 0, where some tangents are zero
+    want = O.fetch_material(ss, prim, bary)
+    mats = c.sc.materials_array()
+    prim_mat = c.sc.prim_mat
+    albedo = np.array([[mats[m].albedo[0], mats[m].albedo[1], mats[m].albedo[2]] for m in prim_mat[prim]], np.float32)
+    rough = np.array([max(mats[m].roughness, 0.1) for m in prim_mat[prim]], np.float32)
+    metal = np.array([mats[m].metallic for m in prim_mat[prim]], np.float32)
+    texels, desc = pack(c.textures)
+    mt = (MatTex * len(c.bindings))()
+    for i, b in enumerate(c.bindings):
+        mt[i] = MatTex(b.get("albedo", -1), b.get("normal", -1), b.get("roughness", -1), b.get("roughness_channel", 0), b.get("metallic", -1), b.get("metallic_channel", 0), -1, 0)
+    lut = srgb_lut()
+    L = emu()
+    L.emu_material_at_hit(O.p(texels), desc, len(c.textures), O.p(lut), mt, O.p(vuv), O.p(prim_mat), O.p(prim), O.p(bary), n, O.p(albedo), O.p(rough), O.p(metal))
+    got = np.concatenate([albedo, rough[:, None], metal[:, None]], 1)
+    assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
+    if case == "channels":  # the roughness clamp fired and let values above it through
+        assert (want[:, 3] == np.float32(0.1)).any() and (want[:, 3] > np.float32(0.1)).any()
+    plain = O.ShadingScene(c.sc, brute=True)
+    n_interp = O.fetch_normal(plain, prim, bary)
+    for quirk in (1, 0):
+        want = O.fetch_normal(ss, prim, bary, hit_shader=bool(quirk))
+        got = n_interp.copy()
+        L.emu_normal_at_hit(O.p(texels), desc, len(c.textures), O.p(lut), mt, O.p(vuv), O.p(vtb), O.p(prim_mat), O.p(prim), O.p(bary), n, quirk, O.p(got))
+        nan_w, nan_g = np.isnan(want), np.isnan(got)
+        assert np.array_equal(nan_w, nan_g)
+        assert np.array_equal(got[~nan_g].view(np.uint32), want[~nan_w].view(np.uint32))

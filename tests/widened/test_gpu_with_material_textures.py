@@ -2,7 +2,9 @@
 scene_descriptor_set.glsl:164-218, normal maps included) through the C ABI against the oracle: the TEX instantiations of the G-buffer producer (all four images bit
 for bit), the reflections and DDGI ray-trace stages (ray lengths / probe distances exact, colours within the shading tolerance) and the
 ground-truth path tracer; removing the textures restores the untextured results.  The arithmetic of the texture functions themselves is
-checked on the CPU (tests/test_textures_cpu.py: host build of csrc/tex_px.cuh == oracle, bit for bit)."""
+checked on the CPU (tests/test_textures_cpu.py: host build of csrc/tex_px.cuh == oracle, bit for bit).  This is one planar-UV scene;
+every textured instantiation (K12 without the DDGI terms and at spp > 1 included) at the sampler's edges is compared in
+tests/test_gpu_textured_kernels.py, on the cases of tests/texture_cases.py."""
 import numpy as np
 import pytest
 
