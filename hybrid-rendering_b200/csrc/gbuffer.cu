@@ -23,8 +23,8 @@ struct GbufScene {
 
 struct GbufParams {
     float vpi[16], vp[16], pvp[16];
-    int   W, H, row0, row1;
-    int   chunk_first, chunk_stride; // chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride of the whole image (rows ignored)
+    int    W, H;
+    RowSet rows;
 };
 
 __device__ __forceinline__ float4 mul_m4(const float* M, V3 p)
@@ -54,9 +54,9 @@ __global__ void __launch_bounds__(64) k_gbuffer_render(BvhDev bvh, GbufScene sc,
 {
     __shared__ int s_stack[2][STACK_SIZE]; // one packet-traversal stack per warp
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int x = (blockIdx.x * 2 + warp) * 8 + (lane & 7);
-    const int y = (P.chunk_stride > 1 ? 8 * (P.chunk_first + ((int)blockIdx.y >> 1) * P.chunk_stride) + 4 * ((int)blockIdx.y & 1) : P.row0 + (int)blockIdx.y * 4) + (lane >> 3);
-    const int y_end = P.chunk_stride > 1 ? P.H : P.row1;
+    int       x, y;
+    P.rows.pixel(x, y);
+    const int  y_end = P.rows.end(P.H);
     const bool in_img = x < P.W && y < P.H && y < y_end;
     V3       N   = det::mk(0.0f, 0.0f, 0.0f);
     uint32_t mid = 0xFFFFFFFFu;
@@ -161,19 +161,17 @@ __global__ void __launch_bounds__(64) k_gbuffer_render(BvhDev bvh, GbufScene sc,
 
 } // namespace
 
-void launch_gbuffer_render(const hr_scene* sc, const hr_frame* f, int W, int H, int row0, int row1, int chunk_first, int chunk_stride, void* gb1, void* gb2, void* gb3,
-                           float* depth, unsigned long long* ray_ctr, cudaStream_t st)
+void launch_gbuffer_render(const hr_scene* sc, const hr_frame* f, int W, int H, RowSet rows, void* gb1, void* gb2, void* gb3, float* depth, unsigned long long* ray_ctr,
+                           cudaStream_t st)
 {
-    const int n_chunks_mine = chunk_stride > 1 ? (((H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0;
-    if (chunk_stride > 1 ? n_chunks_mine <= 0 : row1 <= row0) return;
+    if (rows.empty(H)) return;
     GbufScene gs { sc->d_vnormals, sc->d_prim_inst, sc->d_prim_mat, sc->d_materials };
     GbufParams P;
     memcpy(P.vpi, f->ubo.view_proj_inverse, 64);
     memcpy(P.vp, f->ubo.view_proj, 64);
     memcpy(P.pvp, f->ubo.prev_view_proj, 64);
-    P.W = W; P.H = H; P.row0 = row0; P.row1 = row1;
-    P.chunk_first = chunk_first; P.chunk_stride = chunk_stride;
-    dim3 grid((W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
+    P.W = W; P.H = H; P.rows = rows;
+    const dim3 grid = rows.grid(W, H);
     if (sc->tex.n_textures > 0) k_gbuffer_render<true><<<grid, 64, 0, st>>>(hr_bvh_view(sc), gs, P, (uint32_t*)gb1, (uint2*)gb2, (uint2*)gb3, depth, ray_ctr, sc->tex);
     else k_gbuffer_render<false><<<grid, 64, 0, st>>>(hr_bvh_view(sc), gs, P, (uint32_t*)gb1, (uint2*)gb2, (uint2*)gb3, depth, ray_ctr, sc->tex);
 }

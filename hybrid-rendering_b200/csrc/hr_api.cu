@@ -606,7 +606,7 @@ int hr_gbuffer_stage_render(hr_ctx* ctx, const hr_frame* frame)
     HR_REQUIRE(ctx, !ctx->staged_pending, HR_ERR_INVALID_ARG, "hr_gbuffer_stage_render: a staged frame is already waiting for hr_gbuffer_commit_staged");
     int rc = staging_begin(ctx);
     if (rc != HR_OK) return rc;
-    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, 0, ctx->gb_h, 0, 1, ctx->staging_mip0[0], ctx->staging_mip0[1], ctx->staging_mip0[2],
+    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, RowSet::band(0, ctx->gb_h), ctx->staging_mip0[0], ctx->staging_mip0[1], ctx->staging_mip0[2],
                           (float*)ctx->staging_mip0[3], ctx->gbuf_ray_ctr, ctx->upload_stream);
     ctx->launches++;
     HR_CHECK_LAUNCH(ctx);
@@ -653,7 +653,8 @@ int hr_gbuffer_render(hr_ctx* ctx, int slot, const hr_frame* frame, int row0, in
     HR_REQUIRE(ctx, row0 >= 0 && row1 > row0 && row1 <= ctx->gb_h && row0 % 8 == 0 && (row1 % 8 == 0 || row1 == ctx->gb_h), HR_ERR_INVALID_ARG,
                "hr_gbuffer_render: rows must be multiples of 8 (or end at the image height)");
     GBufSlot& s = use_owned_mip0(ctx, slot);
-    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, row0, row1, 0, 1, s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr, (cudaStream_t)stream);
+    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, RowSet::band(row0, row1), s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr,
+                          (cudaStream_t)stream);
     ctx->launches++;
     HR_CHECK_LAUNCH(ctx);
     return hr_launch_build_mips(ctx, s, ctx->gb_w, ctx->gb_h, (cudaStream_t)stream);
@@ -671,8 +672,8 @@ int hr_gbuffer_render_sharded(hr_ctx* ctx, int slot, const hr_frame* frame, int 
     int b0, b1, r0, r1;
     hr_band(ctx, ctx->gb_h, &b0, &b1);
     hr_extend(b0, b1, round_up8(halo_rows), ctx->gb_h, &r0, &r1);
-    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, r0, r1, 0, 1, s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr, (cudaStream_t)stream);
-    launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, 0, 0, ctx->rank, ctx->world, s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr, (cudaStream_t)stream);
+    for (const RowSet rows : { RowSet::band(r0, r1), RowSet::interleave(ctx->rank, ctx->world) })
+        launch_gbuffer_render(ctx->scene, frame, ctx->gb_w, ctx->gb_h, rows, s.gb1[0], s.gb2[0], s.gb3[0], s.depth[0], ctx->gbuf_ray_ctr, (cudaStream_t)stream);
     ctx->launches += 2;
     HR_CHECK_LAUNCH(ctx);
     return hr_launch_build_mips(ctx, s, ctx->gb_w, ctx->gb_h, (cudaStream_t)stream);

@@ -54,6 +54,29 @@ struct FrameConsts {           // what kernels need from hr_frame (passed by val
 #define HR_RAY_CTR_SLOTS 32
 #define HR_RAY_CTR_STRIDE 4 // unsigned long longs between slots (32 bytes: one sector each)
 
+// The rows a closest-hit ray-trace launch covers (G-buffer producer, K12, path tracer, references): the band [row0, row1), or, when
+// linked ranks trace cooperatively (chunk_stride > 1), the 8-row chunks c = chunk_first + i * chunk_stride of the whole image.
+// Launched as 2-warp CTAs of 16x4 pixels, warp = 8x4 pixel block; a chunk is two CTA rows.
+struct RowSet {
+    int row0, row1, chunk_first, chunk_stride;
+    __host__ __device__ static RowSet band(int r0, int r1) { return { r0, r1, 0, 1 }; }
+    __host__ __device__ static RowSet interleave(int rank, int world) { return { 0, 0, rank, world }; } // world > 1
+    __host__ __device__ int chunk(int i) const { return chunk_first + i * chunk_stride; }
+    int  chunks(int H) const { return chunk_stride > 1 ? (((H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0; }
+    bool empty(int H) const { return chunk_stride > 1 ? chunks(H) <= 0 : row1 <= row0; }
+    dim3 grid(int W, int H) const { return dim3((W + 15) / 16, chunk_stride > 1 ? 2 * chunks(H) : (row1 - row0 + 3) / 4); }
+    // this lane's pixel, and the row limit besides the image's: end(H) = the first row not covered (H for chunks), past_end(y) = y is
+    // past a band's end (never for chunks: the image height bounds them)
+    __device__ __forceinline__ void pixel(int& x, int& y) const
+    {
+        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        x = (blockIdx.x * 2 + warp) * 8 + (lane & 7);
+        y = (chunk_stride > 1 ? 8 * chunk((int)blockIdx.y >> 1) + 4 * ((int)blockIdx.y & 1) : row0 + (int)blockIdx.y * 4) + (lane >> 3);
+    }
+    __device__ __forceinline__ int  end(int H) const { return chunk_stride > 1 ? H : row1; }
+    __device__ __forceinline__ bool past_end(int y) const { return chunk_stride <= 1 && y >= row1; }
+};
+
 // ---- objects ----------------------------------------------------------------------------------------
 #define HR_MAX_RANKS 8
 #define HR_MAX_SHARED 9
@@ -305,17 +328,17 @@ void launch_ddgi_probe_update(const hr_ddgi_uniforms& d, const void* radiance, c
                               void* out_depth, int first_frame, int probe0, int probe1, cudaStream_t st);
 void launch_ddgi_sample_probe_grid(const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms& d, const void* irr, const void* depth, float gi_intensity,
                                    void* out, int row0, int row1, cudaStream_t st);
-void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
-                                  float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
-                                  const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
-                                  int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st); // chunk_stride > 1: only the 8-row chunks c = chunk_first + i * chunk_stride (rows are ignored)
+// The DDGI inputs of a reflections render (refl_gi, hr_api_gi.inc): the DDGI pass's uniforms and the atlases it wrote this frame (null
+// without a usable grid), and the sample_gi / approximate_with_ddgi flags K12 and the reflections reference apply.
+struct ReflGi { const hr_ddgi_uniforms* d; const void* irr; const void* dep; int sample_gi, approx; };
+void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const ReflGi& gi, const hr_reflections_params& prm,
+                                  const void* brdf_lut, const uint8_t* sobol, const uint8_t* srk, void* out, RowSet rows, cudaStream_t st);
 
-// reference.cu (hr_reference_render): samples k0 .. k0 + n - 1 of rows [row0, row1) of the full-resolution G-buffer level g
-void launch_reference_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, uint32_t k0, int n, int row0, int row1,
+// reference.cu (hr_reference_render): samples k0 .. k0 + n - 1 of the band `rows` of the full-resolution G-buffer level g
+void launch_reference_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, uint32_t k0, int n, RowSet rows,
                            uint32_t* count, cudaStream_t st); // kind PASS_SHADOWS (K1: p0 = bias) or PASS_AO (K7: p0 = ray length, p1 = bias)
-void launch_reference_reflections(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
-                                  const hr_reflections_params& prm, int sample_gi, int approximate_with_ddgi, const void* brdf_lut, uint32_t k0, int n, int row0,
-                                  int row1, double* acc, cudaStream_t st);
+void launch_reference_reflections(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const ReflGi& gi, const hr_reflections_params& prm,
+                                  const void* brdf_lut, uint32_t k0, int n, RowSet rows, double* acc, cudaStream_t st);
 // MEAN (R16F from count, or RGBA16F from acc) and STDERR of rows [row0, row1) after n_samples samples
 void launch_reference_resolve(const GBufLevelDev& g, const uint32_t* count, const double* acc, uint32_t n_samples, float sky_value, float power, int row0, int row1,
                               void* mean, void* err, cudaStream_t st);
@@ -371,14 +394,13 @@ int hr_shard_exchange(hr_pass* p, const ExchangeItem* items, int n, cudaStream_t
 void hr_wait_exchange(hr_pass* p, cudaStream_t st);
 
 // ---- kernel launchers (defined in the .cu files) -----------------------------------------------------
-void launch_gbuffer_render(const hr_scene* sc, const hr_frame* f, int W, int H, int row0, int row1, int chunk_first, int chunk_stride, void* gb1, void* gb2, void* gb3,
-                           float* depth, unsigned long long* ray_ctr, cudaStream_t st); // gbuffer.cu
+void launch_gbuffer_render(const hr_scene* sc, const hr_frame* f, int W, int H, RowSet rows, void* gb1, void* gb2, void* gb3, float* depth, unsigned long long* ray_ctr,
+                           cudaStream_t st); // gbuffer.cu
 void launch_deferred(const GBufLevelDev& g, const FrameConsts& fc, const void* shadow, int shadow_channels, const void* ao, const void* reflections, const void* gi,
                      const float* env3, const void* brdf_lut, void* out, int row0, int row1, cudaStream_t st); // deferred.cu
 // rt_shade.cu: ground-truth path tracer
-void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, int row0, int row1,
-                       int chunk_first, int chunk_stride, cudaStream_t st); // rows [row0, row1), or chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride
+void launch_path_trace(const hr_scene* sc, const hr_frame* f, const hr_path_tracer_params& prm, int W, int H, uint32_t num_frames, const void* prev, void* out,
+                       uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, RowSet rows, cudaStream_t st);
 // post.cu: TAA and tone map resolve rows [row0, row1); the blit covers the whole image
 void launch_taa(const GBufLevelDev& g, const void* current, int current_channels, const void* history, const float* jitter_xy, float feedback_min, float feedback_max,
                 int sharpen, void* out, int row0, int row1, cudaStream_t st);

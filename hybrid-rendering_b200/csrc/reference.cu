@@ -2,8 +2,8 @@
 // One thread per pixel of the full-resolution G-buffer runs a loop over `samples` rays of the pass it references: the ray of
 // K1 or K7 (mask_ray, mask_px.cuh, which trace.cu calls too) or K12's sample (refl_ddgi_sample, shade_px.cuh, and refl_trace_shade below),
 // with the same G-buffer inputs and parameters.  Only the random numbers differ: (r0, r1) of global sample k come from the xoroshiro64* stream of gi_common.cuh seeded with (x, y, k),
-// so any split of the samples over renders traces the same rays.  Mapping and CTA size as K1 / K12: warp = 8x4 pixel block,
-// 2-warp CTAs (ray costs are heavy-tailed, trace.cu).
+// so any split of the samples over renders traces the same rays.  Mapping and CTA size as K1 / K12 (RowSet, a band): warp = 8x4 pixel
+// block, 2-warp CTAs (ray costs are heavy-tailed, trace.cu).
 //
 // BUILD NOTE: compiled with -fmad=false, like trace.cu and rt_shade.cu: the rays, the hits and the binary visibilities follow
 // the deterministic chain (det_math.cuh), so the shadows / AO counts equal the CPU oracle's bit for bit.
@@ -12,16 +12,6 @@
 #include "shade_px.cuh"
 
 namespace {
-
-#define REF_CTA_WARPS 2
-
-// pixel (x, y) of the warp's 8x4 block; rows start at row0
-__device__ __forceinline__ void ref_pixel(int row0, int& x, int& y)
-{
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    x = (blockIdx.x * REF_CTA_WARPS + warp) * 8 + (lane & 7);
-    y = row0 + (int)blockIdx.y * 4 + (lane >> 3);
-}
 
 __device__ __forceinline__ void ref_random(int x, int y, uint32_t k, float& r0, float& r1)
 {
@@ -32,11 +22,11 @@ __device__ __forceinline__ void ref_random(int x, int y, uint32_t k, float& r0, 
 
 // MODE 0 = shadows (K1: p0 = bias), 1 = AO (K7: p0 = ray length, p1 = bias).  count[pixel] += unoccluded rays of samples k0 .. k0 + n - 1.
 template <int MODE>
-__global__ void __launch_bounds__(REF_CTA_WARPS * 32) k_reference_mask(GBufLevelDev g, BvhDev bvh, FrameConsts fc, float p0, float p1, uint32_t k0, int n,
-                                                                       int row0, int row1, uint32_t* __restrict__ count)
+__global__ void __launch_bounds__(64) k_reference_mask(GBufLevelDev g, BvhDev bvh, FrameConsts fc, float p0, float p1, uint32_t k0, int n, int row0, int row1,
+                                                       uint32_t* __restrict__ count)
 {
     int x, y;
-    ref_pixel(row0, x, y);
+    RowSet::band(row0, row1).pixel(x, y);
     uint32_t hits = 0, traced = 0;
     if (x < g.W && y < row1)
     {
@@ -81,19 +71,16 @@ __device__ __forceinline__ void refl_trace_shade(const BvhDev& bvh, const ShadeD
     else color = sky;
 }
 
-struct RefReflParams { float bias, trim, gi_intensity, rough_ddgi_intensity; float sky[3]; int sample_gi, approximate_with_ddgi; IblDev ibl; };
-
 // K12's sample: the mirror ray (roughness < 0.05), the DDGI lookup (roughness > 0.75 with approximate_with_ddgi) or the GGX lobe
 // sample, shaded like K12 and clamped to 0.7 per channel.  acc[6 * pixel] += (sum r, g, b, sum of squares r, g, b) in float64.
 // The mirror and DDGI samples do not depend on k: they are evaluated once and added n times.
 template <bool TEX, bool GI>
-__global__ void __launch_bounds__(REF_CTA_WARPS * 32) k_reference_reflections(GBufLevelDev g, BvhDev bvh, ShadeDev sd, FrameConsts fc, hr_ddgi_uniforms d,
-                                                                              gi::AtlasDev at, RefReflParams P, uint32_t k0, int n, int row0, int row1,
-                                                                              double* __restrict__ acc, tex::TexDev T)
+__global__ void __launch_bounds__(64) k_reference_reflections(GBufLevelDev g, BvhDev bvh, ShadeDev sd, FrameConsts fc, hr_ddgi_uniforms d, gi::AtlasDev at,
+                                                              ReflTraceParams P, uint32_t k0, int n, double* __restrict__ acc, tex::TexDev T)
 {
     int x, y;
-    ref_pixel(row0, x, y);
-    if (x >= g.W || y >= row1) return;
+    RowSet::band(P.rows.row0, P.rows.row1).pixel(x, y);
+    if (x >= g.W || y >= P.rows.row1) return;
     const size_t idx   = (size_t)y * g.W + x;
     const float  depth = __ldg(g.depth + idx);
     if (depth == 1.0f) return;
@@ -179,37 +166,28 @@ __global__ void __launch_bounds__(256) k_reference_resolve(GBufLevelDev g, const
 
 } // namespace
 
-static dim3 ref_grid(int W, int row0, int row1) { return dim3(((W + 7) / 8 + REF_CTA_WARPS - 1) / REF_CTA_WARPS, (row1 - row0 + 3) / 4, 1); }
-
-void launch_reference_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, uint32_t k0, int n, int row0, int row1,
+void launch_reference_mask(int kind, const GBufLevelDev& g, const BvhDev& bvh, const FrameConsts& fc, float p0, float p1, uint32_t k0, int n, RowSet rows,
                            uint32_t* count, cudaStream_t st)
 {
-    if (row1 <= row0) return;
+    if (rows.empty(g.H)) return;
     const auto k = kind == PASS_AO ? k_reference_mask<1> : k_reference_mask<0>;
-    k<<<ref_grid(g.W, row0, row1), REF_CTA_WARPS * 32, 0, st>>>(g, bvh, fc, p0, p1, k0, n, row0, row1, count);
+    k<<<rows.grid(g.W, g.H), 64, 0, st>>>(g, bvh, fc, p0, p1, k0, n, rows.row0, rows.row1, count);
 }
 
-void launch_reference_reflections(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
-                                  const hr_reflections_params& prm, int sample_gi, int approximate_with_ddgi, const void* brdf_lut, uint32_t k0, int n, int row0,
-                                  int row1, double* acc, cudaStream_t st)
+void launch_reference_reflections(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const ReflGi& gi, const hr_reflections_params& prm,
+                                  const void* brdf_lut, uint32_t k0, int n, RowSet rows, double* acc, cudaStream_t st)
 {
-    if (row1 <= row0) return;
-    RefReflParams P { prm.bias, prm.trim, prm.gi_intensity, prm.rough_ddgi_intensity, { prm.sky_color[0], prm.sky_color[1], prm.sky_color[2] }, sample_gi,
-                      approximate_with_ddgi, IblDev { (const uint32_t*)brdf_lut, prm.ibl_indirect_specular_intensity } };
-    hr_ddgi_uniforms du;
-    memset(&du, 0, sizeof(du));
-    if (d) du = *d;
-    gi::AtlasDev at { (const uint2*)irr, (const uint32_t*)depth };
-    const bool gi = sample_gi == 1 || approximate_with_ddgi == 1; // K12's GI = false kernel: no DDGI lookups, no IBL term
-    const dim3 grid = ref_grid(g.W, row0, row1);
-#define HR_REF_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, du, at, P, k0, n, row0, row1, acc, sc->tex
+    if (rows.empty(g.H)) return;
+    const ReflLaunch L    = refl_launch(gi, prm, brdf_lut, rows); // K12's GI = false kernel: no DDGI lookups, no IBL term
+    const dim3       grid = rows.grid(g.W, g.H);
+#define HR_REF_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, L.d, L.at, L.P, k0, n, acc, sc->tex
     if (sc->tex.n_textures > 0)
     {
-        if (gi) k_reference_reflections<true, true><<<grid, REF_CTA_WARPS * 32, 0, st>>>(HR_REF_ARGS);
-        else k_reference_reflections<true, false><<<grid, REF_CTA_WARPS * 32, 0, st>>>(HR_REF_ARGS);
+        if (L.gi) k_reference_reflections<true, true><<<grid, 64, 0, st>>>(HR_REF_ARGS);
+        else k_reference_reflections<true, false><<<grid, 64, 0, st>>>(HR_REF_ARGS);
     }
-    else if (gi) k_reference_reflections<false, true><<<grid, REF_CTA_WARPS * 32, 0, st>>>(HR_REF_ARGS);
-    else k_reference_reflections<false, false><<<grid, REF_CTA_WARPS * 32, 0, st>>>(HR_REF_ARGS);
+    else if (L.gi) k_reference_reflections<false, true><<<grid, 64, 0, st>>>(HR_REF_ARGS);
+    else k_reference_reflections<false, false><<<grid, 64, 0, st>>>(HR_REF_ARGS);
 #undef HR_REF_ARGS
 }
 

@@ -67,9 +67,6 @@ __global__ void __launch_bounds__(256) k_ddgi_ray_trace(BvhDev bvh, ShadeDev sd,
     }
 }
 
-struct ReflTraceParams { float bias, trim; int sample_gi, approximate_with_ddgi; float gi_intensity, rough_ddgi_intensity; float sky[3]; int row0, row1;
-                         int chunk_first, chunk_stride; int spp; IblDev ibl; }; // chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
-
 // K12: warp = 8x4 pixel block (coherent reflection rays), 256 threads = 32x8 pixels
 // 2-warp CTAs (16x4 pixels): closest-hit rays + hit shading are heavy-tailed, small CTAs recycle their slots sooner (trace.cu)
 // MULTI = false: exactly the reference's one ray per pixel (straight-line code); true: the spp > 1 extension (sample loop)
@@ -85,11 +82,9 @@ __global__ void __launch_bounds__(64, MINB) k_reflections_ray_trace(GBufLevelDev
                                                                 ReflTraceParams P, const uint8_t* __restrict__ sobol, const uint8_t* __restrict__ srk,
                                                                 uint2* __restrict__ out, tex::TexDev T)
 {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // rows: [row0, row1) or, when the ranks trace cooperatively, the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
-    const int x = blockIdx.x * 16 + warp * 8 + (lane & 7);
-    const int y = (P.chunk_stride > 1 ? 8 * (P.chunk_first + ((int)blockIdx.y >> 1) * P.chunk_stride) + 4 * ((int)blockIdx.y & 1) : P.row0 + (int)blockIdx.y * 4) + (lane >> 3);
-    if (x >= g.W || y >= g.H || (P.chunk_stride <= 1 && y >= P.row1)) return;
+    int x, y;
+    P.rows.pixel(x, y);
+    if (x >= g.W || y >= g.H || P.rows.past_end(y)) return;
     const size_t idx   = (size_t)y * g.W + x;
     const float  depth = __ldg(g.depth + idx);
     if (depth == 1.0f) { out[idx] = pack_h4(0.0f, 0.0f, 0.0f, -1.0f); return; }
@@ -164,7 +159,7 @@ struct PathTraceParams {
     float    sky[3];
     int      W, H;
     unsigned long long* ray_ctr;
-    int      row0, row1, chunk_first, chunk_stride; // chunk_stride > 1: the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
+    RowSet   rows;
 };
 
 __device__ __forceinline__ float4 mat_vec4(const float* M, float x, float y, float z, float w)
@@ -255,12 +250,10 @@ template <bool TEX, bool INDIRECT>
 __global__ void __launch_bounds__(64) k_path_trace(BvhDev bvh, ShadeDev sd, PathTraceParams P, const uint2* __restrict__ prev, uint2* __restrict__ out, uint32_t* __restrict__ out_prim,
                                                    tex::TexDev T, uint32_t* __restrict__ out_hash)
 {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // rows: [row0, row1) or, when the ranks trace cooperatively, the 8-row chunks c = chunk_first + i * chunk_stride of the whole image
-    // (the row mapping of k_reflections_ray_trace).  The RNG is seeded from (x, y, sample): no result depends on the rank.
-    const int x = blockIdx.x * 16 + warp * 8 + (lane & 7);
-    const int y = (P.chunk_stride > 1 ? 8 * (P.chunk_first + ((int)blockIdx.y >> 1) * P.chunk_stride) + 4 * ((int)blockIdx.y & 1) : P.row0 + (int)blockIdx.y * 4) + (lane >> 3);
-    if (x >= P.W || y >= P.H || (P.chunk_stride <= 1 && y >= P.row1)) return;
+    // The RNG is seeded from (x, y, sample): no result depends on the rank.
+    int x, y;
+    P.rows.pixel(x, y);
+    if (x >= P.W || y >= P.H || P.rows.past_end(y)) return;
     const size_t idx = (size_t)y * P.W + x;
     // rgen:56-75
     gi::RNG     rng = gi::rng_init((uint32_t)x, (uint32_t)y, P.num_frames);
@@ -364,55 +357,43 @@ void launch_ddgi_ray_trace(const hr_scene* sc, const hr_ddgi_uniforms& d, const 
     else k_ddgi_ray_trace<false><<<probe1 - probe0, threads, 0, st>>>(hr_bvh_view(sc), shade_view(sc), d, at, light, P, (uint2*)radiance, (uint2*)dirdepth, sc->tex);
 }
 
-void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const hr_ddgi_uniforms* d, const void* irr, const void* depth,
-                                  float bias, float trim, int sample_gi, int approximate_with_ddgi, float gi_intensity, float rough_ddgi_intensity, const float* sky3,
-                                  const uint8_t* sobol, const uint8_t* srk, void* out, int row0, int row1, int chunk_first, int chunk_stride,
-                                  int spp, const void* brdf_lut, float ibl_intensity, cudaStream_t st)
+void launch_reflections_ray_trace(const hr_scene* sc, const GBufLevelDev& g, const FrameConsts& fc, const ReflGi& gi, const hr_reflections_params& prm,
+                                  const void* brdf_lut, const uint8_t* sobol, const uint8_t* srk, void* out, RowSet rows, cudaStream_t st)
 {
-    const int n_chunks_mine = chunk_stride > 1 ? (((g.H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0;
-    if (chunk_stride > 1 ? n_chunks_mine <= 0 : row1 <= row0) return;
-    ReflTraceParams P { bias, trim, sample_gi, approximate_with_ddgi, gi_intensity, rough_ddgi_intensity, { sky3[0], sky3[1], sky3[2] }, row0, row1, chunk_first, chunk_stride, spp,
-                        IblDev { (const uint32_t*)brdf_lut, ibl_intensity } };
-    hr_ddgi_uniforms du;
-    memset(&du, 0, sizeof(du));
-    if (d) du = *d;
-    gi::AtlasDev at { (const uint2*)irr, (const uint32_t*)depth };
-    const bool textured = sc->tex.n_textures > 0; // material textures: the TEX instantiations
-    const bool gi = sample_gi == 1 || approximate_with_ddgi == 1; // the spp > 1 kernels keep both terms behind their flags
-    dim3 grid((g.W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
-    const tex::TexDev& T = sc->tex;
-#define HR_K12_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, du, at, P, sobol, srk, (uint2*)out, T
+    if (rows.empty(g.H)) return;
+    const ReflLaunch L        = refl_launch(gi, prm, brdf_lut, rows); // L.gi: the spp > 1 kernels keep both terms behind their flags
+    const bool       textured = sc->tex.n_textures > 0; // material textures: the TEX instantiations
+    const dim3       grid     = rows.grid(g.W, g.H);
+#define HR_K12_ARGS g, hr_bvh_view(sc), shade_view(sc), fc, L.d, L.at, L.P, sobol, srk, (uint2*)out, sc->tex
     if (textured)
     {
-        if (spp > 1) k_reflections_ray_trace<true, 8, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-        else if (gi) k_reflections_ray_trace<false, 18, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+        if (L.P.spp > 1) k_reflections_ray_trace<true, 8, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+        else if (L.gi) k_reflections_ray_trace<false, 18, true, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
         else k_reflections_ray_trace<false, 24, true, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
     }
-    else if (spp > 1) k_reflections_ray_trace<true, 8, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
-    else if (gi) k_reflections_ray_trace<false, 18, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+    else if (L.P.spp > 1) k_reflections_ray_trace<true, 8, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
+    else if (L.gi) k_reflections_ray_trace<false, 18, false, true><<<grid, 64, 0, st>>>(HR_K12_ARGS);
     else k_reflections_ray_trace<false, 24, false, false><<<grid, 64, 0, st>>>(HR_K12_ARGS);
 #undef HR_K12_ARGS
 }
 
-void launch_path_trace(const hr_scene* sc, const hr_frame* f, int W, int H, uint32_t num_frames, uint32_t max_ray_bounces, float roughness_multiplier, const float* sky3,
-                       int trace_indirect, const void* prev, void* out, uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, int row0, int row1,
-                       int chunk_first, int chunk_stride, cudaStream_t st)
+void launch_path_trace(const hr_scene* sc, const hr_frame* f, const hr_path_tracer_params& prm, int W, int H, uint32_t num_frames, const void* prev, void* out,
+                       uint32_t* out_prim, uint32_t* out_hash, unsigned long long* ray_ctr, RowSet rows, cudaStream_t st)
 {
-    const int n_chunks_mine = chunk_stride > 1 ? (((H + 7) / 8) - chunk_first + chunk_stride - 1) / chunk_stride : 0;
-    if (chunk_stride > 1 ? n_chunks_mine <= 0 : row1 <= row0) return;
+    if (rows.empty(H)) return;
     PathTraceParams P;
     memcpy(P.view_inverse, f->ubo.view_inverse, 64);
     memcpy(P.proj_inverse, f->ubo.proj_inverse, 64);
     P.light = f->ubo.light;
-    P.num_frames = num_frames; P.max_ray_bounces = max_ray_bounces; P.roughness_multiplier = roughness_multiplier;
-    P.sky[0] = sky3[0]; P.sky[1] = sky3[1]; P.sky[2] = sky3[2];
+    P.num_frames = num_frames; P.max_ray_bounces = (uint32_t)prm.max_ray_bounces; P.roughness_multiplier = prm.roughness_multiplier;
+    P.sky[0] = prm.sky_color[0]; P.sky[1] = prm.sky_color[1]; P.sky[2] = prm.sky_color[2];
     P.W = W; P.H = H;
     P.ray_ctr = ray_ctr;
-    P.row0 = row0; P.row1 = row1; P.chunk_first = chunk_first; P.chunk_stride = chunk_stride;
-    dim3 grid((W + 15) / 16, chunk_stride > 1 ? 2 * n_chunks_mine : (row1 - row0 + 3) / 4);
+    P.rows = rows;
+    const dim3 grid = rows.grid(W, H);
 #define HR_PT_ARGS hr_bvh_view(sc), shade_view(sc), P, (const uint2*)prev, (uint2*)out, out_prim, sc->tex
     const bool textured = sc->tex.n_textures > 0; // material textures change the lobe inputs: both indirect forms have a TEX instantiation
-    if (trace_indirect)
+    if (prm.trace_indirect)
     {
         if (textured) k_path_trace<true, true><<<grid, 64, 0, st>>>(HR_PT_ARGS, out_hash);
         else k_path_trace<false, true><<<grid, 64, 0, st>>>(HR_PT_ARGS, out_hash);

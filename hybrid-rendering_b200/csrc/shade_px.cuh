@@ -241,6 +241,24 @@ __device__ __forceinline__ float3 refl_ddgi_sample(const hr_ddgi_uniforms& d, co
     const V3 R = reflect(det::scale(Wo, -1.0f), N);
     return sample_irradiance(d, at, to_f3(Pw), to_f3(R), to_f3(Wo)) * rough_ddgi_intensity;
 }
+
+// K12's launch parameters, which the reflections reference (reference.cu) takes too so that both trace the same sample: the sample
+// parameters of a reflections render (hr_reflections_params with the DDGI terms refl_gi decided), the rows and spp, the DDGI uniforms
+// (zero without a DDGI grid) and atlases, and whether the kernels need the DDGI and IBL terms (GI).  The field order is K12's.
+struct ReflTraceParams { float bias, trim; int sample_gi, approximate_with_ddgi; float gi_intensity, rough_ddgi_intensity; float sky[3]; RowSet rows;
+                         int spp; IblDev ibl; };
+struct ReflLaunch { ReflTraceParams P; hr_ddgi_uniforms d; gi::AtlasDev at; bool gi; };
+inline ReflLaunch refl_launch(const ReflGi& gi, const hr_reflections_params& prm, const void* brdf_lut, RowSet rows)
+{
+    ReflLaunch L {}; // no DDGI grid: zero uniforms
+    L.P = { prm.bias, prm.trim, gi.sample_gi, gi.approx, prm.gi_intensity, prm.rough_ddgi_intensity, { prm.sky_color[0], prm.sky_color[1], prm.sky_color[2] },
+            rows, prm.spp > 1 ? prm.spp : 1, IblDev { (const uint32_t*)brdf_lut, prm.ibl_indirect_specular_intensity } };
+    if (gi.d) L.d = *gi.d;
+    L.at = { (const uint2*)gi.irr, (const uint32_t*)gi.dep };
+    L.gi = gi.sample_gi == 1 || gi.approx == 1;
+    return L;
+}
+
 inline ShadeDev shade_view(const hr_scene* sc)
 {
     ShadeDev s;

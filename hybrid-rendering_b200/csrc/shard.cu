@@ -317,16 +317,16 @@ __global__ void k_peer_wait(const int* __restrict__ ticks, int world, int self, 
     if (r < world && r != self) wait_tick(ticks + r, r, tick, err, 200);
 }
 
-// Interleaved cooperative ray trace (reflections, path tracer): block b copies this rank's chunk c = self + b * world (8 image rows of
-// RGBA16F texels) to every rank that reads those rows; the last block to finish publishes the ray-trace tick.  A rank that owns no
-// chunk still runs PUSH_SPLIT blocks so that its tick is published.
+// Interleaved cooperative ray trace (reflections, path tracer): block b copies the b-th chunk of this rank (RowSet::interleave, 8 image
+// rows of RGBA16F texels) to every rank that reads those rows; the last block to finish publishes the ray-trace tick.  A rank that owns
+// no chunk still runs PUSH_SPLIT blocks so that its tick is published.
 #define PUSH_SPLIT 4
 struct NeedRows { int r0[HR_MAX_RANKS], r1[HR_MAX_RANKS]; };
 __global__ void __launch_bounds__(256) k_rt_push_chunks(PeerPtrs<uint2> imgs, NeedRows need, PeerPtrs<int> ticks, int* __restrict__ ctl, int world, int self, int W, int H,
                                                         int tick)
 {
     // PUSH_SPLIT blocks share one chunk (a chunk is 8 rows x W texels = 245 KB at 4K: one block would walk it in 60 dependent round trips)
-    const int c = self + ((int)blockIdx.x / PUSH_SPLIT) * world, part = (int)blockIdx.x % PUSH_SPLIT, r0 = c * 8, r1 = min(r0 + 8, H);
+    const int c = RowSet::interleave(self, world).chunk((int)blockIdx.x / PUSH_SPLIT), part = (int)blockIdx.x % PUSH_SPLIT, r0 = c * 8, r1 = min(r0 + 8, H);
     if (r0 < H)
         for (int q = 0; q < world; q++)
         {
@@ -519,7 +519,7 @@ int hr_push_chunks(hr_pass* p, int img, int tick, const int* need0, const int* n
         nd.r0[r] = need0[r];
         nd.r1[r] = need1[r];
     }
-    const int n_chunks = (p->H + 7) / 8, mine = (n_chunks - ctx->rank + ctx->world - 1) / ctx->world;
+    const int mine = RowSet::interleave(ctx->rank, ctx->world).chunks(p->H);
     k_rt_push_chunks<<<(mine > 0 ? mine : 1) * PUSH_SPLIT, 256, 0, st>>>(peer_image_ptrs<uint2>(p, img), nd, peer_tick_ptrs(p), p->rt_bounds, ctx->world, ctx->rank,
                                                                         p->W, p->H, tick);
     ctx->launches++;
